@@ -1,4 +1,4 @@
-"""artdeco_b200 — B200-native (sm_100a) kernels behind ARTDECO's hot-path operator surface.
+"""artdeco_b200 — H100-native (sm_90a) kernels behind ARTDECO's hot-path operator surface.
 
 Public operators (same names / argument meaning as the reference's, see each module's docstring):
   ssim.fused_ssim, ssim.FusedSSIMMap, ssim.fusedssim, ssim.fusedssim_backward      (fused_ssim)
@@ -10,7 +10,7 @@ Public operators (same names / argument meaning as the reference's, see each mod
   matching.iter_proj, matching.refine_matches, matching.match   (mast3r_slam_backends + utils_matching)
   optimizers.BaseAdam, optimizers.SparseGaussianAdam   (Reconstruct/scene/optimizers.py: fused step, one-launch add_and_prune)
   legacy.GaussianRasterizer, legacy.rasterize_gaussians  (diff_gaussian_rasterization legacy API, web viewer)
-There is no CPU implementation: every operator raises unless a CUDA sm_100 device and the C-ABI library
+There is no CPU implementation: every operator raises unless a CUDA sm_90 device and the C-ABI library
 ``libartdeco_b200.so`` are available.
 """
 from . import _lib  # noqa: F401

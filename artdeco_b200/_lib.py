@@ -126,9 +126,9 @@ _checked_devices: set[int] = set()
 
 
 def require_cuda(t: torch.Tensor | None = None) -> None:
-    """Fail loudly when there is no sm_100 device: the product path has no CPU implementation."""
+    """Fail loudly when there is no sm_90 device: the product path has no CPU implementation."""
     if not torch.cuda.is_available():
-        raise ArtdecoB200Error("artdeco_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+        raise ArtdecoB200Error("artdeco_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
     if t is not None and not t.is_cuda:
         raise ArtdecoB200Error("expected a CUDA tensor: artdeco_b200 has no CPU implementation")
     dev =t.device.index if (t is not None and t.is_cuda) else torch.cuda.current_device()

@@ -1,4 +1,4 @@
-"""Builds ``libartdeco_b200.so`` (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Builds ``libartdeco_b200.so`` (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
 The library has no torch/pybind dependency: it is plain CUDA runtime + CUB headers, so it can be
 bound from ctypes, cgo, JNI or anything else (see INTEGRATION.md).  Objects are cached by source
@@ -18,7 +18,7 @@ CSRC = PKG_DIR / "csrc"
 BUILD = PKG_DIR / "build"
 LIB_PATH = PKG_DIR / "libartdeco_b200.so"
 
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON_FLAGS = [
     "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
     "--expt-relaxed-constexpr", "-I", str(CSRC), "-I", str(PKG_DIR.parent / "include"),

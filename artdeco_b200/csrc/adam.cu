@@ -83,7 +83,7 @@ ADB_API int adb_adam_update(long long N, long long M, float* param, const float*
     const bool vec = (M % 4 == 0) && ((((uintptr_t)param | (uintptr_t)grad | (uintptr_t)m1 | (uintptr_t)m2 |
                                         (uintptr_t)lr_dev) & 15) == 0);
     const long long work = vec ? N * M / 4 : N * M;
-    const int blocks = (int)((work + 255) / 256 < 148LL * 16 ? (work + 255) / 256 : 148LL * 16);
+    const int blocks = (int)((work + 255) / 256 < 132LL * 16 ? (work + 255) / 256 : 132LL * 16);
     if (vec)
         adam_kernel<4, false><<<blocks, 256, 0, stream>>>(N, M, param, grad, m1, m2, visible, lr_dev, lr_mode, lr_scalar,
                                                          b1, b2, eps, nullptr, 1.f, 0.f);
@@ -105,7 +105,7 @@ ADB_API int adb_adam_update_decay(long long N, long long M, float* param, const 
     const bool vec = (M % 4 == 0) && ((((uintptr_t)param | (uintptr_t)grad | (uintptr_t)m1 | (uintptr_t)m2 |
                                         (uintptr_t)lr) & 15) == 0);
     const long long work = vec ? N * M / 4 : N * M;
-    const int blocks = (int)((work + 255) / 256 < 148LL * 16 ? (work + 255) / 256 : 148LL * 16);
+    const int blocks = (int)((work + 255) / 256 < 132LL * 16 ? (work + 255) / 256 : 132LL * 16);
     if (vec)
         adam_kernel<4, true><<<blocks, 256, 0, stream>>>(N, M, param, grad, m1, m2, visible, lr, 3, 0.f, b1, b2, eps, lr,
                                                         lr_decay, lr_min);

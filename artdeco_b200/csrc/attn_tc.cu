@@ -1,5 +1,5 @@
-// Fused attention on tcgen05: O = softmax(scale * Q K^T) V for one (batch*head, 128-query tile) per CTA, with the
-// score matrix resident in TENSOR MEMORY — S and P never touch HBM.
+// Fused attention on the Hopper tensor cores (wgmma): O = softmax(scale * Q K^T) V for one (batch*head, query group)
+// work item at a time, with the score matrix held in registers — S and P never touch HBM or shared memory.
 //
 // Replaces the reference's materialised attention
 //   attn = (q @ k.transpose(-2,-1)) * scale; attn = attn.softmax(-1); x = attn @ v
@@ -7,25 +7,23 @@
 // the reference runs as three torch kernels with a [B,h,N,N] fp32 tensor written and read twice.
 //
 // Structure (head_dim = 64, keys processed in blocks of 128):
-//   TMA producer warps    Q tile once; K blocks through a 3-stage ring (read twice: see below); V^T blocks through a 3-stage
-//                         ring from a second producer warp.  The loads are LATENCY-bound (~1 us per 32 KB block from L2): with
-//                         every MMA and all of the softmax arithmetic removed the kernel ran only 15 % faster, so ring depth,
-//                         not math, sets the speed
-//   MMA warp (1 thread)   S_j = Q K_j^T  (tcgen05.mma M128 N128 K16, bf16x3 = 12 MMAs) into one of two TMEM S buffers;
-//                         O += P_j V_j   (M128 N64 K16, bf16x3 = 24 MMAs) into a TMEM O accumulator
-//   8 softmax warps       two warps per TMEM lane quarter: thread == (query row, 64-key half of each key block).
-//                         PASS 1 reads every S_j (computed from the bf16 HI parts only: the subtracted maximum only has to
-//                         be close to the true one, softmax is invariant to it) and keeps the row maximum.  PASS 2 recomputes
-//                         S_j in bf16x3, forms p = exp2((s - max) * scale*log2e), accumulates the row sum, and stores its
-//                         64-key half of P_j as packed bf16 (hi, lo) words back into TENSOR MEMORY, over the very columns
-//                         the scores came from (tcgen05.st): P V is a TS-MMA (A operand from TMEM, B = V^T from smem), so P
-//                         costs no shared-memory write, no proxy fence and no operand read bandwidth.  The two halves are
-//                         independent pipeline stages (own full barrier): P V of one half overlaps the exponentials of the
-//                         other and of the next block; an S/P buffer is recycled when the P V products that read it retire.
-//   Two passes instead of an online-softmax rescale: the running-max correction would need a TMEM read-modify-write of O
-//   per key block; recomputing Q K^T costs 12 extra MMAs per block and keeps O a pure accumulate chain.
+//   warp 8 (TMA)          the item's Q tiles once; K blocks through a KST-stage ring (read twice: see below)
+//   warp 9 (TMA)          V^T blocks through a VST-stage ring (own warp so that a full K ring never delays it)
+//   warps 0..7            two consumer warpgroups; warpgroup w owns query rows [64 w, 64 w + 64) of every 128-query tile.
+//                         Per key block and query tile: S = Q K^T with wgmma m64n128k16 (bf16x3 = 12 MMAs) into 64
+//                         registers; a query row lives in the four threads of one quad, so row max / row sum need two
+//                         shuffles.  PASS 1 computes S from the bf16 HI parts only and keeps the row maximum (it only has to
+//                         be close to the true one, softmax is invariant to it).  PASS 2 recomputes S in bf16x3, forms
+//                         p = exp2((s - max) * scale*log2e), accumulates the row sum, and packs P as bf16 (hi, lo) words
+//                         directly in the register A-operand layout of wgmma m64n64k16: O += P V (bf16x3 = 24 MMAs) reads P
+//                         from registers and V^T from shared memory.
+//   Two passes instead of an online-softmax rescale keep O a pure accumulate chain (no per-block rescale of O).
+//   TILES = 1: one 128-query tile per CTA (grid = work items).  TILES = 2: two query tiles share every K / V block
+//   (half the K / V traffic per query) in PERSISTENT CTAs looping over the work items; the next item's Q loads while the
+//   current one finishes.
 // Precision: bf16x3 everywhere (same contract as csrc/gemm_tc.cu); exp via ex2.approx (2 ulp).
 #include "common.cuh"
+#include "hopper.cuh"
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <stdio.h>
@@ -34,90 +32,20 @@
 
 namespace {
 
-constexpr int NT = 352;                  // warp 0 TMA (Q, K), warp 1 MMA (+TMEM alloc), warps 2..9 softmax, warp 10 TMA (V)
-constexpr int KST = 3, VST = 3;          // K / V ring depths: loads are latency-bound (~1 us), keep 3 blocks in flight
+using namespace hopper;
+
+constexpr int NT = 320;                  // warps 0..7 consumers (two warpgroups), warp 8 TMA (Q, K), warp 9 TMA (V^T)
 constexpr int QT = 128, KT = 128, HD = 64;
 constexpr int TILE16 = 128 * 64 * 2;     // [128 rows x 64 cols] bf16 = 16 KB
 constexpr int TILE8 = 64 * 64 * 2;       // [64 rows x 64 cols] bf16 = 8 KB
-constexpr int TMEM_COLS = 512;
-constexpr int O_COL = 256;
 
 struct AttnParams {
-    int Nq, Nk, heads, n_qtiles;
+    int Nq, Nk, heads, n_groups;         // n_groups: query groups of TILES * 128 per (batch*head)
     float scale_log2e;
     __nv_bfloat16* Ohi; __nv_bfloat16* Olo;   // [B, Nq, heads*64]
     int nterms;
-    int dbg;   // diagnostic switches (ADB_ATTN_DBG): 1 no ex2, 2 no lo split, 4 no tmem store, 8 no pass-1 max
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t.reg .pred P1;\n\t"
-        "WAIT_LOOP:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-        "@P1 bra DONE;\n\t"
-        "bra WAIT_LOOP;\n\t"
-        "DONE:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mma(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
-}
-// A operand from TENSOR MEMORY (128 lanes x 8 columns per K=16 step, two bf16 per 32-bit column, k even in the low half)
-__device__ __forceinline__ void tc_mma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;   // SWIZZLE_128B
-    return d;
-}
-__device__ __forceinline__ uint32_t make_idesc(int n) {
-    uint32_t d = 0;
-    d |= 1u << 4; d |= 1u << 7; d |= 1u << 10;
-    d |= (uint32_t)(n >> 3) << 17;
-    d |= (uint32_t)(128 >> 4) << 24;
-    return d;
-}
 // one MUFU.EX2; exp2f() wraps it in a denormal-range rescale (FSETP + 2 predicated FMUL) that softmax weights below 2^-126
 // do not need -- they flush to zero
 __device__ __forceinline__ float ex2_ftz(float x) {
@@ -125,626 +53,262 @@ __device__ __forceinline__ float ex2_ftz(float x) {
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+__device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
+    const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
+    return *reinterpret_cast<const uint32_t*>(&h2);
 }
 
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-          "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-          "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-          "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
-}
+// Ring depths and shared-memory map (bytes, 1024-aligned tiles) per variant: Q tiles (hi, lo), K stages (hi, lo),
+// V^T stages [2 key-chunks x (hi, lo) x 8 KB].  Both variants use 224 KB of the 227 KB a block may have.
+template <int TILES>
+struct Layout {
+    static constexpr int KST = 3, VST = TILES == 1 ? 3 : 2;
+    static constexpr int OFF_Q = 0;
+    static constexpr int OFF_K = OFF_Q + TILES * 2 * TILE16;
+    static constexpr int OFF_V = OFF_K + KST * 2 * TILE16;
+    static constexpr int OFF_BAR = OFF_V + VST * 4 * TILE8;
+    static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
+    enum { B_QFULL = 0, B_QEMPTY = 1, B_KFULL = 2, B_KEMPTY = B_KFULL + KST, B_VFULL = B_KEMPTY + KST,
+           B_VEMPTY = B_VFULL + VST, B_COUNT = B_VEMPTY + VST };
+};
 
-// shared memory map (bytes, 1024-aligned tiles)
-constexpr int OFF_Q = 0;                       // Q hi, Q lo            2 x 16 KB
-constexpr int OFF_K = OFF_Q + 2 * TILE16;      // KST stages x (K hi, K lo)   96 KB
-constexpr int OFF_V = OFF_K + KST * 2 * TILE16;  // V^T: VST stages x [2 key-chunks x (hi, lo) x 8 KB] = 96 KB
-constexpr int OFF_BAR = OFF_V + VST * 4 * TILE8; // barriers (P lives in tensor memory, in the columns of the S block it came from)
-constexpr int OFF_RED = OFF_BAR + 256;         // [2 halves][128 rows] floats: row max / row sum exchange
-constexpr int SMEM_BYTES = OFF_RED + 2 * 128 * 4 + 1024;
-
-enum { B_QFULL = 0, B_KFULL = 1, B_KEMPTY = B_KFULL + KST, B_VFULL = B_KEMPTY + KST, B_VEMPTY = B_VFULL + VST,
-       B_SFULL = B_VEMPTY + VST, B_SEMPTY = B_SFULL + 2, B_PFULL = B_SEMPTY + 2 /*[S buffer][half]*/, B_OFULL = B_PFULL + 4,
-       B_COUNT = B_OFULL + 1 };
-
+template <int TILES>
 __global__ void __launch_bounds__(NT, 1)
 attn_fused_kernel(const __grid_constant__ CUtensorMap mQhi, const __grid_constant__ CUtensorMap mQlo,
                   const __grid_constant__ CUtensorMap mKhi, const __grid_constant__ CUtensorMap mKlo,
                   const __grid_constant__ CUtensorMap mVhi, const __grid_constant__ CUtensorMap mVlo,
-                  const AttnParams p) {
+                  const AttnParams p, const int n_items) {
+    using L = Layout<TILES>;
+    constexpr int KST = L::KST, VST = L::VST;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint64_t* bar = (uint64_t*)(smem + OFF_BAR);
-    uint32_t* tmem_ptr = (uint32_t*)(bar + B_COUNT);
+    uint64_t* bar = (uint64_t*)(smem + L::OFF_BAR);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const bool x3 = p.nterms == 3;
-    const int qt = blockIdx.x % p.n_qtiles, bh = blockIdx.x / p.n_qtiles;
-    const int q0 = qt * QT;
     const int nb = (p.Nk + KT - 1) / KT;
     const uint32_t kstage_bytes = (x3 ? 2 : 1) * TILE16, v_bytes = (x3 ? 4 : 2) * TILE8;
 
-    if (warp == 0 && lane == 0) {
-        mbar_init(bar + B_QFULL, 1);
-        for (int s = 0; s < KST; ++s) { mbar_init(bar + B_KFULL + s, 1); mbar_init(bar + B_KEMPTY + s, 1); }
-        for (int s = 0; s < VST; ++s) { mbar_init(bar + B_VFULL + s, 1); mbar_init(bar + B_VEMPTY + s, 1); }
-        for (int s = 0; s < 2; ++s) {
-            // an S buffer is free again after 8 softmax-warp arrivals + 1 from the MMA warp: a plain arrive in pass 1, the
-            // commit of the P V product that read P out of the same columns in pass 2
-            mbar_init(bar + B_SFULL + s, 1); mbar_init(bar + B_SEMPTY + s, 9);
-            // one P-full barrier per (S buffer, half): a single barrier per half could advance two phases before the MMA warp
-            // looks (softmax of block j+1 only needs S_{j+1}, which is issued before P V of block j) and the parity wait would hang
-            mbar_init(bar + B_PFULL + 2 * s, 4); mbar_init(bar + B_PFULL + 2 * s + 1, 4);
-        }
-        mbar_init(bar + B_OFULL, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "n"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-
-    if (warp == 0) {
-        // ===== TMA producer =====
-        if (elect_one()) {
-            mbar_expect_tx(bar + B_QFULL, (x3 ? 2 : 1) * TILE16);
-            tma_load_3d(smem + OFF_Q, &mQhi, bar + B_QFULL, 0, q0, bh);
-            if (x3) tma_load_3d(smem + OFF_Q + TILE16, &mQlo, bar + B_QFULL, 0, q0, bh);
-            for (int it = 0; it < 2 * nb; ++it) {          // K blocks: pass 1 then pass 2
-                const int j = it % nb, s = it % KST;
-                mbar_wait(bar + B_KEMPTY + s, ((it / KST) & 1) ^ 1);
-                uint8_t* st = smem + OFF_K + s * 2 * TILE16;
-                const bool lo = x3 && it >= nb;             // pass 1 multiplies the hi parts only
-                mbar_expect_tx(bar + B_KFULL + s, lo ? kstage_bytes : (uint32_t)TILE16);
-                tma_load_3d(st, &mKhi, bar + B_KFULL + s, 0, j * KT, bh);
-                if (lo) tma_load_3d(st + TILE16, &mKlo, bar + B_KFULL + s, 0, j * KT, bh);
-            }
-        }
-    } else if (warp == 10) {
-        // ===== TMA producer for V^T (pass 2 only; own warp so that a full K ring never delays it and vice versa) =====
-        if (elect_one()) {
-            for (int j = 0; j < nb; ++j) {                  // two 64-key chunks per block
-                const int vs = j % VST;
-                mbar_wait(bar + B_VEMPTY + vs, ((j / VST) & 1) ^ 1);
-                mbar_expect_tx(bar + B_VFULL + vs, v_bytes);
-                uint8_t* vt = smem + OFF_V + vs * 4 * TILE8;
-                tma_load_3d(vt, &mVhi, bar + B_VFULL + vs, j * KT, 0, bh);
-                tma_load_3d(vt + TILE8, &mVhi, bar + B_VFULL + vs, j * KT + 64, 0, bh);
-                if (x3) {
-                    tma_load_3d(vt + 2 * TILE8, &mVlo, bar + B_VFULL + vs, j * KT, 0, bh);
-                    tma_load_3d(vt + 3 * TILE8, &mVlo, bar + B_VFULL + vs, j * KT + 64, 0, bh);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        const uint32_t idS = make_idesc(128), idO = make_idesc(64);
-        const uint32_t qa = smem_u32(smem + OFF_Q);
-        mbar_wait(bar + B_QFULL, 0);
-        tc_fence_after();
-        auto issue_S = [&](int it, bool full) {   // S[it&1] = Q K^T for K ring slot it&1 (full: bf16x3, else hi x hi)
-            const int s = it & 1, ks = it % KST;
-            mbar_wait(bar + B_KFULL + ks, (it / KST) & 1);
-            mbar_wait(bar + B_SEMPTY + s, ((it >> 1) & 1) ^ 1);
-            tc_fence_after();
-            if (elect_one()) {
-                const uint32_t ka = smem_u32(smem + OFF_K + ks * 2 * TILE16);
-                const uint64_t dQh = make_smem_desc(qa), dQl = make_smem_desc(qa + TILE16);
-                const uint64_t dKh = make_smem_desc(ka), dKl = make_smem_desc(ka + TILE16);
-                const uint32_t td = tmem_base + s * 128;
-#pragma unroll
-                for (int k = 0; k < HD / 16; ++k) {
-                    const uint64_t adv = (uint64_t)((k * 32) >> 4);
-                    tc_mma(td, dQh + adv, dKh + adv, idS, k ? 1u : 0u);
-                    if (x3 && full && !(p.dbg & 32)) {
-                        tc_mma(td, dQh + adv, dKl + adv, idS, 1u);
-                        tc_mma(td, dQl + adv, dKh + adv, idS, 1u);
-                    }
-                }
-                tc_commit(bar + B_KEMPTY + ks);
-                tc_commit(bar + B_SFULL + s);
-                if (!full) mbar_arrive(bar + B_SEMPTY + s);     // pass 1: nothing of ours reads this buffer later
-            }
-            __syncwarp();
-        };
-        for (int it = 0; it < nb; ++it) issue_S(it, false);         // pass 1
-        issue_S(nb, true);                                           // first S of pass 2
-        for (int j = 0; j < nb; ++j) {
-            if (j + 1 < nb) issue_S(nb + j + 1, true);               // overlap the next S with this block's softmax
-            const int vs = j % VST;
-            mbar_wait(bar + B_VFULL + vs, (j / VST) & 1);
-#pragma unroll 1
-            for (int c = 0; c < 2; ++c) {                            // two 64-key halves, each its own pipeline stage
-                mbar_wait(bar + B_PFULL + 2 * ((nb + j) & 1) + c, (j >> 1) & 1);
-                tc_fence_after();
-                if (elect_one()) {
-                    const uint32_t va = smem_u32(smem + OFF_V + vs * 4 * TILE8);
-                    const uint32_t td = tmem_base + O_COL;
-                    // P half c of this block sits in the S buffer's own columns: hi words [c*64, +32), lo words [c*64+32, +32)
-                    const uint32_t ph = tmem_base + ((nb + j) & 1) * 128 + c * 64, pl = ph + 32;
-                    const uint64_t dVh = make_smem_desc(va + c * TILE8), dVl = make_smem_desc(va + (2 + c) * TILE8);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint64_t adv = (uint64_t)((k * 32) >> 4);
-                        tc_mma_ts(td, ph + k * 8, dVh + adv, idO, (j | c | k) ? 1u : 0u);
-                        if (x3 && !(p.dbg & 16)) {
-                            tc_mma_ts(td, ph + k * 8, dVl + adv, idO, 1u);
-                            tc_mma_ts(td, pl + k * 8, dVh + adv, idO, 1u);
-                        }
-                    }
-                    if (c == 1) {
-                        tc_commit(bar + B_VEMPTY + vs);
-                        tc_commit(bar + B_SEMPTY + ((nb + j) & 1));     // S/P buffer reusable once these products retire
-                        if (j == nb - 1) tc_commit(bar + B_OFULL);
-                    }
-                }
-                __syncwarp();
-            }
-        }
-    } else if (warp < 10) {
-        // ===== softmax / epilogue warps: thread == (query row, 64-key half) =====
-        const int q = warp & 3;                    // TMEM lane quarter
-        const int half = (warp - 2) >> 2;          // which 64 keys of every 128-key block (and which 32 columns of O)
-        const int row = q * 32 + lane;
-        const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-        float* red = reinterpret_cast<float*>(smem + OFF_RED);
-        float m = -3.0e38f;
-        // PASS 1: row maximum of the raw scores
-        for (int it = 0; it < nb; ++it) {
-            const int s = it & 1;
-            mbar_wait(bar + B_SFULL + s, (it >> 1) & 1);
-            tc_fence_after();
-#pragma unroll 1
-            for (int g2 = 0; g2 < 2; ++g2) {
-                uint32_t r[32];
-                tmem_ld32(tmem_base + lane_addr + s * 128 + half * 64 + g2 * 32, r);
-                const int kbase = it * KT + half * 64 + g2 * 32;
-                if (!(p.dbg & 8)) {
-#pragma unroll
-                    for (int e = 0; e < 32; ++e)
-                        if (kbase + e < p.Nk) m = fmaxf(m, __uint_as_float(r[e]));
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar + B_SEMPTY + s);
-        }
-        red[half * 128 + row] = m;
-        asm volatile("bar.sync 1, 256;" ::: "memory");          // the 8 softmax warps only
-        m = fmaxf(m, red[(half ^ 1) * 128 + row]);
-        asm volatile("bar.sync 1, 256;" ::: "memory");          // red[] is reused for the row sums below
-        // PASS 2: p = exp2((s - m) * scale*log2e) -> packed bf16 (hi, lo) words stored back to tensor memory; row sum
-        float l = 0.f;
-        const float c1 = p.scale_log2e, c0 = -m * p.scale_log2e;
-        for (int j = 0; j < nb; ++j) {
-            const int it = nb + j, s = it & 1;
-            mbar_wait(bar + B_SFULL + s, (it >> 1) & 1);
-            tc_fence_after();
-            // all 64 scores of this half first: the P words overwrite the same columns
-            uint32_t r[64];
-            tmem_ld32_nowait(tmem_base + lane_addr + s * 128 + half * 64, r);
-            tmem_ld32_nowait(tmem_base + lane_addr + s * 128 + half * 64 + 32, r + 32);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            const int kbase = j * KT + half * 64;
-            const bool tail = kbase + 64 > p.Nk;        // only the last key block can hold padded keys
-            uint32_t hw[32], lw[32];
-#pragma unroll
-            for (int e = 0; e < 32; ++e) {
-                float a = fmaf(__uint_as_float(r[2 * e]), c1, c0);
-                float b = fmaf(__uint_as_float(r[2 * e + 1]), c1, c0);
-                if (!(p.dbg & 1)) { a = ex2_ftz(a); b = ex2_ftz(b); }
-                if (tail) {
-                    if (kbase + 2 * e >= p.Nk) a = 0.f;
-                    if (kbase + 2 * e + 1 >= p.Nk) b = 0.f;
-                }
-                l += a + b;
-                // packed split: one cvt.rn.bf16x2 for the hi pair, shift/mask to widen it back, one for the lo pair
-                const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
-                const uint32_t hb = *reinterpret_cast<const uint32_t*>(&h2);
-                hw[e] = hb;
-                lw[e] = 0;
-                if (!(p.dbg & 2)) {
-                    const __nv_bfloat162 l2 = __floats2bfloat162_rn(a - __uint_as_float(hb << 16), b - __uint_as_float(hb & 0xffff0000u));
-                    lw[e] = *reinterpret_cast<const uint32_t*>(&l2);
-                }
-            }
-            if (!(p.dbg & 4)) {
-                tmem_st32(tmem_base + lane_addr + s * 128 + half * 64, hw);
-                if (x3) tmem_st32(tmem_base + lane_addr + s * 128 + half * 64 + 32, lw);
-                asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) { mbar_arrive(bar + B_SEMPTY + s); mbar_arrive(bar + B_PFULL + 2 * s + half); }
-        }
-        red[half * 128 + row] = l;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        l += red[(half ^ 1) * 128 + row];
-        // epilogue: O / l -> bf16 split in [B, Nq, heads*64]; this warp writes columns [half*32, half*32+32)
-        mbar_wait(bar + B_OFULL, 0);
-        tc_fence_after();
-        const float inv = 1.0f / l;
-        const int qrow = q0 + row;
-        const int b = bh / p.heads, hh = bh % p.heads;
-        const size_t o = ((size_t)b * p.Nq + qrow) * (size_t)(p.heads * HD) + (size_t)hh * HD;
-        {
-            const int c = half;
-            uint32_t r[32];
-            tmem_ld32(tmem_base + lane_addr + O_COL + c * 32, r);
-            if (qrow < p.Nq) {
-#pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    uint32_t hw[4], lw[4];
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const float a = __uint_as_float(r[g * 8 + 2 * e]) * inv, bb = __uint_as_float(r[g * 8 + 2 * e + 1]) * inv;
-                        const __nv_bfloat16 ah = __float2bfloat16_rn(a), bh2 = __float2bfloat16_rn(bb);
-                        const __nv_bfloat16 al = __float2bfloat16_rn(a - __bfloat162float(ah));
-                        const __nv_bfloat16 bl = __float2bfloat16_rn(bb - __bfloat162float(bh2));
-                        hw[e] = (uint32_t)__bfloat16_as_ushort(ah) | ((uint32_t)__bfloat16_as_ushort(bh2) << 16);
-                        lw[e] = (uint32_t)__bfloat16_as_ushort(al) | ((uint32_t)__bfloat16_as_ushort(bl) << 16);
-                    }
-                    *reinterpret_cast<uint4*>(p.Ohi + o + c * 32 + g * 8) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                    if (p.Olo) *reinterpret_cast<uint4*>(p.Olo + o + c * 32 + g * 8) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-                }
-            }
-        }
-        tc_fence_before();
+    if (warp == 8 && lane == 0) {
+        mbar_init(bar + L::B_QFULL, 1); mbar_init(bar + L::B_QEMPTY, 8);
+        for (int s = 0; s < KST; ++s) { mbar_init(bar + L::B_KFULL + s, 1); mbar_init(bar + L::B_KEMPTY + s, 8); }
+        for (int s = 0; s < VST; ++s) { mbar_init(bar + L::B_VFULL + s, 1); mbar_init(bar + L::B_VEMPTY + s, 8); }
+        mbar_init_fence();
     }
     __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
-    }
-}
 
-// =====================================================================================================================
-// Variant 2 (opt-in, ADB_ATTN_KERNEL=2): TWO query tiles (256 queries) per CTA sharing every K / V^T block, in a PERSISTENT
-// CTA that loops over (batch*head, tile pair) work items.  Motivation (profiles/r01_attn_ablation.md): variant 1 is bound by
-// L2->SM traffic (80 KB of K/V per 128 queries per key block) and by a 5.7 us per-CTA fixed cost that nothing overlaps.
-// Here each K/V block serves 256 queries, and the epilogue of one item overlaps the first pass of the next.
-//   TMEM   S_a [0,128)  S_b [128,256)  O_a [256,320)  O_b [320,384): no second S buffer per tile -- the two tiles ping-pong
-//          (the MMA warp computes S_b while the softmax warps of tile a work, and so on); P overwrites S in place as above.
-//   warps  0: TMA Q + K   1: MMA   2..5: softmax/epilogue of tile a (thread == one query row, all 128 keys of a block,
-//          processed as two 64-key halves)   6..9: the same for tile b   10: TMA V^T
-//   hazards on S_x (written by the S MMA, read by softmax, overwritten by P, read by the P V MMA, overwritten by the next S):
-//          tcgen05.mma instructions execute in issue order, so issuing S_x(n+1) after P V_x(n) needs no barrier; the only
-//          handshakes are S-full (MMA -> softmax) and S-done (softmax -> MMA: scores read in pass 1 / P stored in pass 2).
-//   all barrier phases run on counters that continue across work items.
-// STATUS: compiled for sm_100a and reviewed, NOT YET RUN ON HARDWARE (the round's GPU budget was spent); therefore opt-in.
-// =====================================================================================================================
-constexpr int K2ST = 3, V2ST = 2;
-constexpr int OFF2_Q = 0;                                   // Q_a hi, Q_a lo, Q_b hi, Q_b lo        64 KB
-constexpr int OFF2_K = OFF2_Q + 4 * TILE16;                 // K2ST x (K hi, K lo)                   96 KB
-constexpr int OFF2_V = OFF2_K + K2ST * 2 * TILE16;          // V2ST x [2 chunks x (hi, lo) x 8 KB]   64 KB
-constexpr int OFF2_BAR = OFF2_V + V2ST * 4 * TILE8;
-constexpr int SMEM2_BYTES = OFF2_BAR + 256 + 1024;
-enum { C_QFULL = 0, C_QEMPTY = 1, C_KFULL = 2, C_KEMPTY = C_KFULL + K2ST, C_VFULL = C_KEMPTY + K2ST, C_VEMPTY = C_VFULL + V2ST,
-       C_SFULL = C_VEMPTY + V2ST, C_SDONE = C_SFULL + 2, C_OFULL = C_SDONE + 2, C_OEMPTY = C_OFULL + 2, C_COUNT = C_OEMPTY + 2 };
-
-__global__ void __launch_bounds__(NT, 1)
-attn_fused2_kernel(const __grid_constant__ CUtensorMap mQhi, const __grid_constant__ CUtensorMap mQlo,
-                   const __grid_constant__ CUtensorMap mKhi, const __grid_constant__ CUtensorMap mKlo,
-                   const __grid_constant__ CUtensorMap mVhi, const __grid_constant__ CUtensorMap mVlo,
-                   const AttnParams p, const int n_items, const int n_pairs) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint64_t* bar = (uint64_t*)(smem + OFF2_BAR);
-    uint32_t* tmem_ptr = (uint32_t*)(bar + C_COUNT);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const bool x3 = p.nterms == 3;
-    const int nb = (p.Nk + KT - 1) / KT;
-    const uint32_t q_bytes = (x3 ? 4 : 2) * TILE16, kstage_bytes = (x3 ? 2 : 1) * TILE16, v_bytes = (x3 ? 4 : 2) * TILE8;
-
-    if (warp == 0 && lane == 0) {
-        mbar_init(bar + C_QFULL, 1); mbar_init(bar + C_QEMPTY, 1);
-        for (int s = 0; s < K2ST; ++s) { mbar_init(bar + C_KFULL + s, 1); mbar_init(bar + C_KEMPTY + s, 1); }
-        for (int s = 0; s < V2ST; ++s) { mbar_init(bar + C_VFULL + s, 1); mbar_init(bar + C_VEMPTY + s, 1); }
-        for (int x = 0; x < 2; ++x) {
-            mbar_init(bar + C_SFULL + x, 1); mbar_init(bar + C_SDONE + x, 4);
-            mbar_init(bar + C_OFULL + x, 1); mbar_init(bar + C_OEMPTY + x, 4);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "n"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-
-    if (warp == 0) {
-        // ===== TMA producer: Q pair once per item, K blocks for both passes =====
-        if (elect_one()) {
+    if (warp == 8) {
+        // ===== TMA producer: the item's Q tiles, then K blocks for both passes =====
+        if (lane == 0) {
             uint32_t kc = 0, wi = 0;
             for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++wi) {
-                const int bh = item / n_pairs, q0 = (item % n_pairs) * 2 * QT;
-                mbar_wait(bar + C_QEMPTY, (wi & 1) ^ 1);               // every S product of the previous item has retired
-                mbar_expect_tx(bar + C_QFULL, q_bytes);
-                tma_load_3d(smem + OFF2_Q, &mQhi, bar + C_QFULL, 0, q0, bh);
-                tma_load_3d(smem + OFF2_Q + 2 * TILE16, &mQhi, bar + C_QFULL, 0, q0 + QT, bh);
-                if (x3) {
-                    tma_load_3d(smem + OFF2_Q + TILE16, &mQlo, bar + C_QFULL, 0, q0, bh);
-                    tma_load_3d(smem + OFF2_Q + 3 * TILE16, &mQlo, bar + C_QFULL, 0, q0 + QT, bh);
+                const int bh = item / p.n_groups, q0 = (item % p.n_groups) * TILES * QT;
+                mbar_wait(bar + L::B_QEMPTY, (wi & 1) ^ 1);         // every S product of the previous item has retired
+                mbar_expect_tx(bar + L::B_QFULL, TILES * kstage_bytes);
+                for (int t = 0; t < TILES; ++t) {
+                    tma_load_3d(smem + L::OFF_Q + t * 2 * TILE16, &mQhi, bar + L::B_QFULL, 0, q0 + t * QT, bh);
+                    if (x3) tma_load_3d(smem + L::OFF_Q + t * 2 * TILE16 + TILE16, &mQlo, bar + L::B_QFULL, 0, q0 + t * QT, bh);
                 }
-                for (int it = 0; it < 2 * nb; ++it, ++kc) {
-                    const int j = it % nb, s = kc % K2ST;
-                    mbar_wait(bar + C_KEMPTY + s, ((kc / K2ST) & 1) ^ 1);
-                    uint8_t* st = smem + OFF2_K + s * 2 * TILE16;
-                    const bool lo = x3 && it >= nb;
-                    mbar_expect_tx(bar + C_KFULL + s, lo ? kstage_bytes : (uint32_t)TILE16);
-                    tma_load_3d(st, &mKhi, bar + C_KFULL + s, 0, j * KT, bh);
-                    if (lo) tma_load_3d(st + TILE16, &mKlo, bar + C_KFULL + s, 0, j * KT, bh);
+                for (int it = 0; it < 2 * nb; ++it, ++kc) {          // pass 1 then pass 2
+                    const int j = it % nb, s = kc % KST;
+                    mbar_wait(bar + L::B_KEMPTY + s, ((kc / KST) & 1) ^ 1);
+                    uint8_t* st = smem + L::OFF_K + s * 2 * TILE16;
+                    const bool lo = x3 && it >= nb;                  // pass 1 multiplies the hi parts only
+                    mbar_expect_tx(bar + L::B_KFULL + s, lo ? kstage_bytes : (uint32_t)TILE16);
+                    tma_load_3d(st, &mKhi, bar + L::B_KFULL + s, 0, j * KT, bh);
+                    if (lo) tma_load_3d(st + TILE16, &mKlo, bar + L::B_KFULL + s, 0, j * KT, bh);
                 }
             }
         }
-    } else if (warp == 10) {
-        // ===== TMA producer: V^T blocks (second pass only) =====
-        if (elect_one()) {
+        return;
+    }
+    if (warp == 9) {
+        // ===== TMA producer for V^T (pass 2 only): two 64-key chunks per block =====
+        if (lane == 0) {
             uint32_t vc = 0;
             for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-                const int bh = item / n_pairs;
+                const int bh = item / p.n_groups;
                 for (int j = 0; j < nb; ++j, ++vc) {
-                    const int vs = vc % V2ST;
-                    mbar_wait(bar + C_VEMPTY + vs, ((vc / V2ST) & 1) ^ 1);
-                    mbar_expect_tx(bar + C_VFULL + vs, v_bytes);
-                    uint8_t* vt = smem + OFF2_V + vs * 4 * TILE8;
-                    tma_load_3d(vt, &mVhi, bar + C_VFULL + vs, j * KT, 0, bh);
-                    tma_load_3d(vt + TILE8, &mVhi, bar + C_VFULL + vs, j * KT + 64, 0, bh);
+                    const int vs = vc % VST;
+                    mbar_wait(bar + L::B_VEMPTY + vs, ((vc / VST) & 1) ^ 1);
+                    mbar_expect_tx(bar + L::B_VFULL + vs, v_bytes);
+                    uint8_t* vt = smem + L::OFF_V + vs * 4 * TILE8;
+                    tma_load_3d(vt, &mVhi, bar + L::B_VFULL + vs, j * KT, 0, bh);
+                    tma_load_3d(vt + TILE8, &mVhi, bar + L::B_VFULL + vs, j * KT + 64, 0, bh);
                     if (x3) {
-                        tma_load_3d(vt + 2 * TILE8, &mVlo, bar + C_VFULL + vs, j * KT, 0, bh);
-                        tma_load_3d(vt + 3 * TILE8, &mVlo, bar + C_VFULL + vs, j * KT + 64, 0, bh);
+                        tma_load_3d(vt + 2 * TILE8, &mVlo, bar + L::B_VFULL + vs, j * KT, 0, bh);
+                        tma_load_3d(vt + 3 * TILE8, &mVlo, bar + L::B_VFULL + vs, j * KT + 64, 0, bh);
                     }
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        const uint32_t idS = make_idesc(128), idO = make_idesc(64);
-        const uint32_t qa = smem_u32(smem + OFF2_Q);
-        uint32_t kc = 0, vc = 0, wi = 0;
-        uint32_t sc[2] = {0u, 0u};            // S products issued so far per tile == index of the next S-full / S-done phase
-        // S_x(sc[x]) = Q_x K^T of the K stage `ks`; waits until the previous contents of S_x have been consumed
-        auto issue_S = [&](int x, int ks, bool full) {
-            if (sc[x] > 0) mbar_wait(bar + C_SDONE + x, (sc[x] - 1) & 1);
-            tc_fence_after();
-            if (elect_one()) {
-                const uint32_t ka = smem_u32(smem + OFF2_K + ks * 2 * TILE16);
-                const uint64_t dQh = make_smem_desc(qa + x * 2 * TILE16), dQl = make_smem_desc(qa + x * 2 * TILE16 + TILE16);
-                const uint64_t dKh = make_smem_desc(ka), dKl = make_smem_desc(ka + TILE16);
-                const uint32_t td = tmem_base + x * 128;
+        return;
+    }
+
+    // ===== consumers =====
+    // accumulator element i of this thread: row 16 (warp % 4) + lane / 4 + 8 h with h = (i / 2) % 2 (of the warpgroup's 64),
+    // column 8 (i / 4) + 2 (lane % 4) + i % 2
+    const int wg = warp >> 2;
+    const int rq = (warp & 3) * 16 + (lane >> 2), cq = 2 * (lane & 3);
+    const uint32_t qa = smem_u32(smem + L::OFF_Q) + wg * (TILE16 / 2);
+    uint32_t kc = 0, vc = 0, wi = 0;
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++wi) {
+        const int bh = item / p.n_groups, q0 = (item % p.n_groups) * TILES * QT;
+        mbar_wait(bar + L::B_QFULL, wi & 1);
+        float S[64];
+        // S = Q_t K^T of K ring slot ks (full: bf16x3, else hi x hi)
+        auto score = [&](int t, int ks, bool full) {
+            const uint32_t ka = smem_u32(smem + L::OFF_K + ks * 2 * TILE16);
+            const uint64_t dQh = make_smem_desc(qa + t * 2 * TILE16), dQl = make_smem_desc(qa + t * 2 * TILE16 + TILE16);
+            const uint64_t dKh = make_smem_desc(ka), dKl = make_smem_desc(ka + TILE16);
+#pragma unroll
+            for (int i = 0; i < 64; ++i) S[i] = 0.f;
+            fence_regs(S);
+            wgmma_fence();
+            if (full) {
 #pragma unroll
                 for (int k = 0; k < HD / 16; ++k) {
                     const uint64_t adv = (uint64_t)((k * 32) >> 4);
-                    tc_mma(td, dQh + adv, dKh + adv, idS, k ? 1u : 0u);
-                    if (x3 && full) {
-                        tc_mma(td, dQh + adv, dKl + adv, idS, 1u);
-                        tc_mma(td, dQl + adv, dKh + adv, idS, 1u);
-                    }
+                    wgmma_m64n128k16_ss(S, dQh + adv, dKh + adv);
+                    wgmma_m64n128k16_ss(S, dQh + adv, dKl + adv);
+                    wgmma_m64n128k16_ss(S, dQl + adv, dKh + adv);
                 }
-                tc_commit(bar + C_SFULL + x);
+            } else {
+#pragma unroll
+                for (int k = 0; k < HD / 16; ++k) {
+                    const uint64_t adv = (uint64_t)((k * 32) >> 4);
+                    wgmma_m64n128k16_ss(S, dQh + adv, dKh + adv);
+                }
             }
-            __syncwarp();
-            ++sc[x];
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(S);
         };
-        for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++wi) {
-            mbar_wait(bar + C_QFULL, wi & 1);
-            // ---- pass 1: hi x hi scores for the row maxima ----
-            for (int it = 0; it < nb; ++it, ++kc) {
-                const int ks = kc % K2ST;
-                mbar_wait(bar + C_KFULL + ks, (kc / K2ST) & 1);
-                issue_S(0, ks, false);
-                issue_S(1, ks, false);
-                if (elect_one()) tc_commit(bar + C_KEMPTY + ks);
-                __syncwarp();
-            }
-            // ---- pass 2: S in bf16x3, P V; software-pipelined so that S_x(j+1) is queued right behind P V_x(j) ----
-            {
-                const int ks = kc % K2ST;
-                mbar_wait(bar + C_KFULL + ks, (kc / K2ST) & 1);
-                issue_S(0, ks, true);
-                issue_S(1, ks, true);
-                if (elect_one()) tc_commit(bar + C_KEMPTY + ks);
-                __syncwarp();
-                ++kc;
-            }
-            for (int j = 0; j < nb; ++j, ++vc) {
-                const int vs = vc % V2ST;
-                mbar_wait(bar + C_VFULL + vs, (vc / V2ST) & 1);
-                const bool more = j + 1 < nb;
-                const int ks = kc % K2ST;
-                if (more) mbar_wait(bar + C_KFULL + ks, (kc / K2ST) & 1);
-#pragma unroll 1
-                for (int x = 0; x < 2; ++x) {
-                    mbar_wait(bar + C_SDONE + x, (sc[x] - 1) & 1);                       // P_x(j) is in tensor memory
-                    if (j == 0) mbar_wait(bar + C_OEMPTY + x, (wi & 1) ^ 1);               // previous item's O_x has been read out
-                    tc_fence_after();
-                    if (elect_one()) {
-                        const uint32_t va = smem_u32(smem + OFF2_V + vs * 4 * TILE8);
-                        const uint32_t td = tmem_base + O_COL + x * 64;
+        // PASS 1: row maxima of the raw hi x hi scores
+        float m[TILES][2];
 #pragma unroll
-                        for (int c = 0; c < 2; ++c) {
-                            const uint32_t ph = tmem_base + x * 128 + c * 64, pl = ph + 32;
-                            const uint64_t dVh = make_smem_desc(va + c * TILE8), dVl = make_smem_desc(va + (2 + c) * TILE8);
+        for (int t = 0; t < TILES; ++t) m[t][0] = m[t][1] = -3.0e38f;
+        for (int it = 0; it < nb; ++it, ++kc) {
+            const int ks = kc % KST;
+            mbar_wait(bar + L::B_KFULL + ks, (kc / KST) & 1);
 #pragma unroll
-                            for (int k = 0; k < 4; ++k) {
-                                const uint64_t adv = (uint64_t)((k * 32) >> 4);
-                                tc_mma_ts(td, ph + k * 8, dVh + adv, idO, (j | c | k) ? 1u : 0u);
-                                if (x3) {
-                                    tc_mma_ts(td, ph + k * 8, dVl + adv, idO, 1u);
-                                    tc_mma_ts(td, pl + k * 8, dVh + adv, idO, 1u);
-                                }
-                            }
-                        }
-                        if (x == 1) tc_commit(bar + C_VEMPTY + vs);
-                        if (!more) tc_commit(bar + C_OFULL + x);
-                    }
-                    __syncwarp();
-                    if (more) issue_S(x, ks, true);            // in-order tensor pipe: runs after the P V_x(j) just queued
-                }
-                if (more) {
-                    if (elect_one()) tc_commit(bar + C_KEMPTY + ks);
-                    __syncwarp();
-                    ++kc;
-                } else {
-                    if (elect_one()) tc_commit(bar + C_QEMPTY);   // the last S products of this item are queued: Q may be replaced
-                    __syncwarp();
-                }
+            for (int t = 0; t < TILES; ++t) {
+                score(t, ks, false);
+                const int kbase = it * KT + cq;
+#pragma unroll
+                for (int i = 0; i < 64; ++i)
+                    if (kbase + 8 * (i >> 2) + (i & 1) < p.Nk) m[t][(i >> 1) & 1] = fmaxf(m[t][(i >> 1) & 1], S[i]);
             }
-        }
-    } else if (warp < 10) {
-        // ===== softmax / epilogue warps: tile x, thread == query row =====
-        const int x = (warp - 2) >> 2, q = warp & 3;
-        const int row = q * 32 + lane;
-        const uint32_t s_addr = tmem_base + ((uint32_t)(q * 32) << 16) + x * 128;
-        const uint32_t o_addr = tmem_base + ((uint32_t)(q * 32) << 16) + O_COL + x * 64;
-        uint32_t n = 0, wi = 0;                 // n: S_x products consumed so far (== phase index of S-full / S-done)
-        for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++wi) {
-            const int bh = item / n_pairs, q0 = (item % n_pairs) * 2 * QT + x * QT;
-            float m = -3.0e38f;
-            for (int it = 0; it < nb; ++it, ++n) {
-                mbar_wait(bar + C_SFULL + x, n & 1);
-                tc_fence_after();
-#pragma unroll 1
-                for (int c = 0; c < 4; ++c) {
-                    uint32_t r[32];
-                    tmem_ld32(s_addr + c * 32, r);
-                    const int kbase = it * KT + c * 32;
-#pragma unroll
-                    for (int e = 0; e < 32; ++e)
-                        if (kbase + e < p.Nk) m = fmaxf(m, __uint_as_float(r[e]));
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar + C_SDONE + x);
-            }
-            float l = 0.f;
-            const float c1 = p.scale_log2e, c0 = -m * p.scale_log2e;
-            for (int j = 0; j < nb; ++j, ++n) {
-                mbar_wait(bar + C_SFULL + x, n & 1);
-                tc_fence_after();
-#pragma unroll 1
-                for (int half = 0; half < 2; ++half) {
-                    // the P words of this half land in the columns its own scores came from; the other half is untouched
-                    uint32_t r[64];
-                    tmem_ld32_nowait(s_addr + half * 64, r);
-                    tmem_ld32_nowait(s_addr + half * 64 + 32, r + 32);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                    const int kbase = j * KT + half * 64;
-                    const bool tail = kbase + 64 > p.Nk;
-                    uint32_t hw[32], lw[32];
-#pragma unroll
-                    for (int e = 0; e < 32; ++e) {
-                        float a = ex2_ftz(fmaf(__uint_as_float(r[2 * e]), c1, c0));
-                        float b = ex2_ftz(fmaf(__uint_as_float(r[2 * e + 1]), c1, c0));
-                        if (tail) {
-                            if (kbase + 2 * e >= p.Nk) a = 0.f;
-                            if (kbase + 2 * e + 1 >= p.Nk) b = 0.f;
-                        }
-                        l += a + b;
-                        const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
-                        const uint32_t hb = *reinterpret_cast<const uint32_t*>(&h2);
-                        const __nv_bfloat162 l2 = __floats2bfloat162_rn(a - __uint_as_float(hb << 16), b - __uint_as_float(hb & 0xffff0000u));
-                        hw[e] = hb;
-                        lw[e] = *reinterpret_cast<const uint32_t*>(&l2);
-                    }
-                    tmem_st32(s_addr + half * 64, hw);
-                    if (x3) tmem_st32(s_addr + half * 64 + 32, lw);
-                }
-                asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar + C_SDONE + x);
-            }
-            // epilogue: O_x / l -> bf16 split in [B, Nq, heads*64]; overlaps the first pass of the next item
-            mbar_wait(bar + C_OFULL + x, wi & 1);
-            tc_fence_after();
-            const float inv = 1.0f / l;
-            const int qrow = q0 + row;
-            const int b = bh / p.heads, hh = bh % p.heads;
-            const size_t o = ((size_t)b * p.Nq + qrow) * (size_t)(p.heads * HD) + (size_t)hh * HD;
-#pragma unroll 1
-            for (int c = 0; c < 2; ++c) {
-                uint32_t r[32];
-                tmem_ld32(o_addr + c * 32, r);
-                if (qrow < p.Nq) {
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        uint32_t hw[4], lw[4];
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const float a = __uint_as_float(r[g * 8 + 2 * e]) * inv, bb = __uint_as_float(r[g * 8 + 2 * e + 1]) * inv;
-                            const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, bb);
-                            const uint32_t hb = *reinterpret_cast<const uint32_t*>(&h2);
-                            const __nv_bfloat162 l2 = __floats2bfloat162_rn(a - __uint_as_float(hb << 16), bb - __uint_as_float(hb & 0xffff0000u));
-                            hw[e] = hb;
-                            lw[e] = *reinterpret_cast<const uint32_t*>(&l2);
-                        }
-                        *reinterpret_cast<uint4*>(p.Ohi + o + c * 32 + g * 8) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                        if (p.Olo) *reinterpret_cast<uint4*>(p.Olo + o + c * 32 + g * 8) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-                    }
-                }
-            }
-            tc_fence_before();
             __syncwarp();
-            if (lane == 0) mbar_arrive(bar + C_OEMPTY + x);
+            if (lane == 0) mbar_arrive(bar + L::B_KEMPTY + ks);
         }
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
+        float c0[TILES][2], l[TILES][2], O[TILES][32];
+        const float c1 = p.scale_log2e;
+#pragma unroll
+        for (int t = 0; t < TILES; ++t)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float v = m[t][h];
+                v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+                v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+                c0[t][h] = -v * c1;
+                l[t][h] = 0.f;
+            }
+#pragma unroll
+        for (int t = 0; t < TILES; ++t)
+#pragma unroll
+            for (int i = 0; i < 32; ++i) O[t][i] = 0.f;
+        // PASS 2: p = exp2((s - m) * scale*log2e) packed as bf16 (hi, lo) A fragments; O += P V; row sums
+        for (int j = 0; j < nb; ++j, ++kc, ++vc) {
+            const int ks = kc % KST, vs = vc % VST;
+            mbar_wait(bar + L::B_KFULL + ks, (kc / KST) & 1);
+            mbar_wait(bar + L::B_VFULL + vs, (vc / VST) & 1);
+            const uint32_t va = smem_u32(smem + L::OFF_V + vs * 4 * TILE8);
+            const int kbase = j * KT + cq;
+            const bool tail = j * KT + KT > p.Nk;            // only the last key block can hold padded keys
+#pragma unroll
+            for (int t = 0; t < TILES; ++t) {
+                score(t, ks, x3);
+                if (t == TILES - 1 && j == nb - 1) {            // the item's last S products have retired: Q may be replaced
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(bar + L::B_QEMPTY);
+                }
+                uint32_t ph[32], pl[32];
+#pragma unroll
+                for (int i = 0; i < 64; i += 2) {
+                    const int h = (i >> 1) & 1;
+                    float a = ex2_ftz(fmaf(S[i], c1, c0[t][h]));
+                    float b = ex2_ftz(fmaf(S[i + 1], c1, c0[t][h]));
+                    if (tail) {
+                        const int key = kbase + 8 * (i >> 2);
+                        if (key >= p.Nk) a = 0.f;
+                        if (key + 1 >= p.Nk) b = 0.f;
+                    }
+                    l[t][h] += a + b;
+                    // packed split: one cvt.rn.bf16x2 for the hi pair, shift/mask to widen it back, one for the lo pair
+                    const uint32_t hb = pack_bf16(a, b);
+                    ph[i >> 1] = hb;
+                    pl[i >> 1] = pack_bf16(a - __uint_as_float(hb << 16), b - __uint_as_float(hb & 0xffff0000u));
+                }
+                fence_regs(ph);
+                fence_regs(pl);
+                fence_regs(O[t]);
+                wgmma_fence();
+                // k-step kk covers keys [16 kk, 16 kk + 16) of the block: A words 4 kk .. 4 kk + 3, V^T chunk kk / 4
+                if (x3) {
+#pragma unroll
+                    for (int kk = 0; kk < KT / 16; ++kk) {
+                        const uint32_t vchunk = va + (kk >> 2) * TILE8;
+                        const uint64_t adv = (uint64_t)(((kk & 3) * 32) >> 4);
+                        const uint64_t dVh = make_smem_desc(vchunk) + adv, dVl = make_smem_desc(vchunk + 2 * TILE8) + adv;
+                        wgmma_m64n64k16_rs(O[t], ph + 4 * kk, dVh);
+                        wgmma_m64n64k16_rs(O[t], ph + 4 * kk, dVl);
+                        wgmma_m64n64k16_rs(O[t], pl + 4 * kk, dVh);
+                    }
+                } else {
+#pragma unroll
+                    for (int kk = 0; kk < KT / 16; ++kk) {
+                        const uint64_t adv = (uint64_t)(((kk & 3) * 32) >> 4);
+                        wgmma_m64n64k16_rs(O[t], ph + 4 * kk, make_smem_desc(va + (kk >> 2) * TILE8) + adv);
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs(O[t]);
+                fence_regs(ph);
+                fence_regs(pl);
+            }
+            __syncwarp();
+            if (lane == 0) { mbar_arrive(bar + L::B_KEMPTY + ks); mbar_arrive(bar + L::B_VEMPTY + vs); }
+        }
+        // epilogue: O / l -> bf16 split in [B, Nq, heads*64]
+        const int b = bh / p.heads, hh = bh % p.heads;
+#pragma unroll
+        for (int t = 0; t < TILES; ++t)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float sum = l[t][h];
+                sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+                sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+                const float inv = 1.0f / sum;
+                const int qrow = q0 + t * QT + wg * 64 + rq + 8 * h;
+                if (qrow >= p.Nq) continue;
+                const size_t o = ((size_t)b * p.Nq + qrow) * (size_t)(p.heads * HD) + (size_t)hh * HD + cq;
+#pragma unroll
+                for (int g = 0; g < 8; ++g) {
+                    const float a = O[t][4 * g + 2 * h] * inv, bb = O[t][4 * g + 2 * h + 1] * inv;
+                    const uint32_t hb = pack_bf16(a, bb);
+                    *reinterpret_cast<uint32_t*>(p.Ohi + o + 8 * g) = hb;
+                    if (p.Olo)
+                        *reinterpret_cast<uint32_t*>(p.Olo + o + 8 * g) =
+                            pack_bf16(a - __uint_as_float(hb << 16), bb - __uint_as_float(hb & 0xffff0000u));
+                }
+            }
     }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn get_encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = (EncodeTiledFn)p;
-    }
-    return fn;
-}
 // bf16 [batch][rows][cols] (cols contiguous); box = 64 cols x box_rows x 1, SWIZZLE_128B
 int make_map(CUtensorMap* map, const void* ptr, long long batch, int rows, int cols, long long ld, int box_rows) {
-    EncodeTiledFn fn = get_encode_fn();
+    hopper::EncodeTiledFn fn = hopper::get_encode_fn();
     if (!fn) { adb_set_error_msg("cuTensorMapEncodeTiled driver entry point unavailable"); return ADB_ERR_CUDA; }
     cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)batch};
     cuuint64_t strides[2] = {(cuuint64_t)ld * 2, (cuuint64_t)rows * ld * 2};
@@ -762,7 +326,7 @@ int make_map(CUtensorMap* map, const void* ptr, long long batch, int rows, int c
 // O[b, n, h*64 + d] = sum_k softmax_k(scale * <Q[b,h,n,:], K[b,h,k,:]>) * V[b,h,k,d]   (head_dim 64)
 //   Q: bf16 split [B*heads, Nq, 64];  K: [B*heads, Nk, 64];  Vt: [B*heads, 64, Nkpad] (Nkpad % 8 == 0, zero padded);
 //   O: bf16 split [B, Nq, heads*64].  *_lo all non-NULL selects bf16x3.
-// 0 = automatic (default; env ADB_ATTN_KERNEL overrides at load), 1 = one query tile per CTA, 2 = two query tiles per
+// 0 = automatic (default, currently variant 1; env ADB_ATTN_KERNEL overrides at load), 1 = one query tile per CTA, 2 = two query tiles per
 // persistent CTA.  Returns the previous setting.  Both variants produce the same values to rounding (tests/test_gemm.py).
 static std::atomic<int> g_attn_variant{getenv("ADB_ATTN_KERNEL") ? atoi(getenv("ADB_ATTN_KERNEL")) : 0};
 ADB_API int adb_attention_set_variant(int variant) {
@@ -791,41 +355,36 @@ ADB_API int adb_attention_bf16(int B, int heads, int Nq, int Nk, int Nkpad, cons
         if ((rc = make_map(&mVl, Vt_lo, bh, 64, Nkpad, Nkpad, 64))) return rc;
     }
     AttnParams p;
-    p.Nq = Nq; p.Nk = Nk; p.heads = heads; p.n_qtiles = adb_cdiv(Nq, QT);
+    p.Nq = Nq; p.Nk = Nk; p.heads = heads;
     p.scale_log2e = scale * 1.4426950408889634f;
     p.Ohi = (__nv_bfloat16*)O_hi; p.Olo = (__nv_bfloat16*)O_lo; p.nterms = x3 ? 3 : 1;
-    static const int dbg = getenv("ADB_ATTN_DBG") ? atoi(getenv("ADB_ATTN_DBG")) : 0;
-    p.dbg = dbg;
     static AdbDeviceOnce once;
     int num_sms = 0;
     {
         const int rc = once.ensure([]() -> int {
-            ADB_CUDA(cudaFuncSetAttribute(attn_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-            ADB_CUDA(cudaFuncSetAttribute(attn_fused2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM2_BYTES));
+            ADB_CUDA(cudaFuncSetAttribute(attn_fused_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Layout<1>::SMEM_BYTES));
+            ADB_CUDA(cudaFuncSetAttribute(attn_fused_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Layout<2>::SMEM_BYTES));
             return ADB_OK;
         }, &num_sms);
         if (rc != ADB_OK) return rc;
     }
-    // Kernel choice.  Variant 2 (two query tiles per persistent CTA) halves the K/V stream per query but its work items are
-    // twice as long, so it wins when its item count quantises well onto the SMs.  Measured on B200 (tools/bench_attn.py,
-    // profiles/r02_attention_variants.md): one variant-2 item costs ~1.75x a variant-1 CTA; pick the smaller wave count.
+    // Kernel choice.  Variant 2 (two query tiles per persistent CTA) halves the K/V stream per query, but at 320 threads its
+    // two O accumulators exceed the 168-register budget (ptxas serialises part of its wgmma and spills): measured on an H100
+    // SXM (400 W), variant 1 is faster at every MASt3R shape (e.g. 16x16 heads x 1024 tokens: 435 vs 537 us; 8x12 x 768:
+    // 118 vs 165 us), so the automatic choice is variant 1.
+    const long long n1 = bh * adb_cdiv(Nq, QT), n2 = bh * adb_cdiv(Nq, 2 * QT);
+    ADB_REQUIRE(n1 < 2147483647LL, "adb_attention_bf16: too many work items");
     int variant = g_attn_variant.load(std::memory_order_relaxed);
-    if (variant == 0) {
-        const long long n1 = bh * p.n_qtiles, n2 = bh * adb_cdiv(Nq, 2 * QT);
-        const long long w1 = (n1 + num_sms - 1) / num_sms, w2 = (n2 + num_sms - 1) / num_sms;
-        variant = (10 * w1 >= 17 * w2) ? 2 : 1;
-    }
+    if (variant == 0) variant = 1;
     if (variant == 2) {
-        const int n_pairs = adb_cdiv(Nq, 2 * QT);
-        const long long items = bh * n_pairs;
-        ADB_REQUIRE(items < 2147483647LL, "adb_attention_bf16: too many work items");
-        const int grid2 = (int)(items < num_sms ? items : num_sms);
-        attn_fused2_kernel<<<grid2, NT, SMEM2_BYTES, stream>>>(mQh, mQl, mKh, mKl, mVh, mVl, p, (int)items, n_pairs);
-        ADB_CHECK_LAUNCH("attn_fused2_kernel");
+        p.n_groups = adb_cdiv(Nq, 2 * QT);
+        const int grid = (int)(n2 < num_sms ? n2 : num_sms);
+        attn_fused_kernel<2><<<grid, NT, Layout<2>::SMEM_BYTES, stream>>>(mQh, mQl, mKh, mKl, mVh, mVl, p, (int)n2);
+        ADB_CHECK_LAUNCH("attn_fused_kernel<2>");
         return ADB_OK;
     }
-    const long long grid = bh * p.n_qtiles;
-    attn_fused_kernel<<<(unsigned)grid, NT, SMEM_BYTES, stream>>>(mQh, mQl, mKh, mKl, mVh, mVl, p);
-    ADB_CHECK_LAUNCH("attn_fused_kernel");
+    p.n_groups = adb_cdiv(Nq, QT);
+    attn_fused_kernel<1><<<(unsigned)n1, NT, Layout<1>::SMEM_BYTES, stream>>>(mQh, mQl, mKh, mKl, mVh, mVl, p, (int)n1);
+    ADB_CHECK_LAUNCH("attn_fused_kernel<1>");
     return ADB_OK;
 }

@@ -90,7 +90,7 @@ ADB_API int adb_compact_gather(long long n_keep, long long n_ext, const int32_t*
         if (wds > max_words) max_words = wds;
     }
     long long bx = (max_words + 255) / 256;
-    if (bx > 148LL * 8) bx = 148LL * 8;
+    if (bx > 132LL * 8) bx = 132LL * 8;
     dim3 grid((unsigned)bx, n_tensors);
     compact_gather_kernel<<<grid, 256, 0, stream>>>(n_keep, n_ext, src_of, tab);
     ADB_CHECK_LAUNCH("compact_gather_kernel");

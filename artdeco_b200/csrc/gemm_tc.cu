@@ -1,4 +1,4 @@
-// Batched GEMM / implicit-GEMM 3x3 convolution on the 5th-generation tensor cores:
+// Batched GEMM / implicit-GEMM 3x3 convolution on the Hopper tensor cores (wgmma):
 //     D = act(alpha * A * B^T + bias) + residual
 //
 // This is the one dense-contraction engine of the MASt3R path: every nn.Linear / q@k^T / attn@v of
@@ -7,38 +7,43 @@
 // convolutions of the DPT head croco/models/dpt_block.py:79-142,356-410.  The reference runs them as fp32 (TF32)
 // cuBLAS / cuDNN calls.
 //
-// sm_100a structure (hand-written PTX, no CUTLASS):
-//   * PERSISTENT: one CTA per SM walks a static round-robin list of 128x128 output tiles;
-//   * operands are bf16, K-major, staged by TMA (cp.async.bulk.tensor, SWIZZLE_128B) into a multi-stage
-//     shared-memory ring guarded by full/empty mbarriers; the producer runs ahead across tile boundaries;
-//   * one elected thread issues tcgen05.mma.cta_group::1.kind::f16 (M=128, N=128, K=16); the fp32 accumulator
-//     lives in TENSOR MEMORY, DOUBLE-BUFFERED (2 x 128 columns) so the epilogue of tile i overlaps the main
-//     loop of tile i+1; tcgen05.commit releases ring slots and publishes finished accumulators;
-//   * eight epilogue warps (two per TMEM lane quarter, 64 columns each) read the accumulator with
-//     tcgen05.ld.32x32b.x32, PROMOTE partial sums to round-to-nearest fp32 registers every 16 k-blocks (the tensor
-//     core's accumulator truncates: its error grows linearly with the chain length), then apply alpha / bias /
-//     GELU(erf) or ReLU / residual and write fp32 and/or a bf16 (hi, lo) split, one full 128 B line per thread;
+// sm_90a structure (hand-written PTX, no CUTLASS):
+//   * one CTA per 128x128 output tile; operands are bf16, K-major, staged by TMA (cp.async.bulk.tensor, SWIZZLE_128B)
+//     into a multi-stage shared-memory ring guarded by full/empty mbarriers, filled by one producer warp;
+//   * two consumer warpgroups, 64 rows each, issue wgmma.mma_async m64n128k16 (bf16 in, fp32 accumulator in registers)
+//     straight from the swizzled ring; one k-block's MMAs stay in flight while the next are issued;
+//   * the accumulator is PROMOTED to a round-to-nearest fp32 register sum every KCHUNK_KB k-blocks (the tensor core's
+//     accumulation error grows linearly with the chain length);
+//   * epilogue: the 128x128 fp32 tile is restaged through shared memory (over the drained ring) so that each thread
+//     owns 64 consecutive columns of one output row, then alpha / bias / GELU(erf) or ReLU / residual are applied and
+//     fp32 and/or a bf16 (hi, lo) split written as full 128 B lines;
 //   * "bf16x3": with the lo operands the kernel accumulates A_hi*B_hi + A_hi*B_lo + A_lo*B_hi into the same
-//     TMEM accumulator (~16 mantissa bits per operand, error ~1e-5): single-pass bf16 or TF32 (the reference's
+//     accumulator (~16 mantissa bits per operand, error ~1e-5): single-pass bf16 or TF32 (the reference's
 //     own GPU mode) cannot hold the north-star's 1e-4 pointmap tolerance over 36 layers;
 //   * CONV MODE: A is an NHWC activation described by a 4-D tensor map; a tile is a Wb x Hb pixel rectangle
 //     and K-block (tap, channel chunk) is ONE shifted TMA box load — out-of-image taps are zero-filled by the
 //     TMA unit, which is exactly the conv's zero padding; no im2col buffer exists.
-// Warp roles: warp 0 = TMA producer, warp 1 = MMA issuer, warp 2 = TMEM allocator, warps 4..11 = epilogue.
+// Warp roles: warps 0..7 = two consumer warpgroups (MMA + epilogue), warp 8 = TMA producer.
 #include "common.cuh"
+#include "hopper.cuh"
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <stdio.h>
 
 namespace {
 
+using namespace hopper;
+
 constexpr int BM = 128, BN = 128, BK = 64;    // BK * 2 B = 128 B = one swizzle row
 constexpr int TILE_BYTES = BM * BK * 2;       // 16 KB (A and B tiles have the same shape)
-constexpr int UMMA_K = 16;
-constexpr int NTHREADS = 384;                 // 4 control warps + 8 epilogue warps
-constexpr int TMEM_COLS = 256;                // two 128-column accumulators
-constexpr int MAX_STAGES = 8;
-constexpr int KCHUNK_KB = 8;                 // k-blocks (of 64) accumulated in TMEM before promotion to registers
+constexpr int MMA_K = 16;
+constexpr int NCONSUMER = 256;                // two warpgroups
+constexpr int NTHREADS = NCONSUMER + 32;      // + the TMA producer warp
+constexpr int RING_BYTES = 192 * 1024;        // 6 stages of (A, B) or 3 of (A_hi, B_hi, A_lo, B_lo)
+constexpr int KCHUNK_KB = 8;                  // k-blocks (of 64) accumulated by the tensor core before promotion
+constexpr int STG_LD = BN + 4;                // fp32 row pitch of the epilogue restaging tile
+constexpr int SMEM_BYTES = RING_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+static_assert(BM * STG_LD * 4 <= RING_BYTES, "epilogue staging must fit over the ring");
 
 struct GemmParams {
     int M, N, K;
@@ -65,99 +70,26 @@ struct GemmParams {
     __nv_bfloat16* rope_hi[2]; __nv_bfloat16* rope_lo[2];
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t.reg .pred P1;\n\t"
-        "WAIT_LOOP:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-        "@P1 bra DONE;\n\t"
-        "bra WAIT_LOOP;\n\t"
-        "DONE:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mma(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-
-// K-major, SWIZZLE_128B operand tile: rows of 128 B, 8-row groups 1024 B apart (SBO), LBO unused.
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3fff);        // start address
-    d |= (uint64_t)1 << 16;                            // leading byte offset (ignored for swizzled K-major)
-    d |= (uint64_t)(1024 >> 4) << 32;                  // stride byte offset
-    d |= (uint64_t)1 << 46;                            // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                            // SWIZZLE_128B
-    return d;
-}
-
-// kind::f16, A = B = BF16 (K-major), D = F32, M = 128, N = 128
-__device__ __forceinline__ uint32_t make_idesc() {
-    uint32_t d = 0;
-    d |= 1u << 4;                 // c_format = F32
-    d |= 1u << 7;                 // a_format = BF16
-    d |= 1u << 10;                // b_format = BF16
-    d |= (uint32_t)(BN >> 3) << 17;
-    d |= (uint32_t)(BM >> 4) << 24;
-    return d;
-}
-
 __device__ __forceinline__ float gelu_erf(float v) { return 0.5f * v * (1.0f + erff(v * 0.70710678118654752f)); }
 
-// 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256): one full 32 B sector per lane per instruction
+// 32 B per thread as two 128-bit accesses: one full sector per lane
 __device__ __forceinline__ void st_v8(float* p, const float* v) {
-    asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]),
-                 "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7]) : "memory");
+    reinterpret_cast<float4*>(p)[0] = make_float4(v[0], v[1], v[2], v[3]);
+    reinterpret_cast<float4*>(p)[1] = make_float4(v[4], v[5], v[6], v[7]);
 }
 __device__ __forceinline__ void st_v8_b32(void* p, const uint32_t* w) {
-    asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]),
-                 "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]) : "memory");
+    reinterpret_cast<uint4*>(p)[0] = make_uint4(w[0], w[1], w[2], w[3]);
+    reinterpret_cast<uint4*>(p)[1] = make_uint4(w[4], w[5], w[6], w[7]);
 }
 __device__ __forceinline__ void ld_v8_nc(const float* p, float* v) {
-    asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];" : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]),
-                 "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]) : "l"(p));
+    const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p) + 1);
+    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
 }
 
 struct TileCoord {
     int bz, mt, nt;
 };
-__device__ __forceinline__ TileCoord decode_tile(const GemmParams& p, int tile, int tiles_m, int tiles_n) {
+__device__ __forceinline__ TileCoord decode_tile(int tile, int tiles_m, int tiles_n) {
     TileCoord c;
     c.nt = tile % tiles_n;
     const int r = tile / tiles_n;
@@ -166,8 +98,129 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmParams& p, int tile, 
     return c;
 }
 
+// Epilogue of one thread: output row `trow` of the tile, columns [n0, n0 + 64) held in acc[2][32].
 // ROPE: the epilogue variant of adb_gemm_bf16_rope (own instantiation so that its extra live values do not cost the plain
 // GEMM registers); it has no residual / activation / split-output paths.
+template <bool ROPE>
+__device__ __forceinline__ void store_row(const GemmParams& p, float (&acc)[2][32], int trow, bool conv, int x0, int y0,
+                                          int m0, int n0, size_t dbase, size_t obase, size_t rbase, bool vec_ok) {
+    long long row;
+    if (conv) {
+        const int yy = y0 + trow / p.conv_wb, xx = x0 + trow % p.conv_wb;
+        row = (yy < p.conv_H && xx < p.conv_W) ? (long long)yy * p.conv_W + xx : -1;
+    } else {
+        row = m0 + trow < p.M ? m0 + trow : -1;
+    }
+    if (row < 0) return;
+#pragma unroll
+    for (int g = 0; g < 2; ++g) {
+        const int c0 = n0 + g * 32;
+        if (c0 >= p.N) continue;
+        float (&v)[32] = acc[g];      // finished accumulators are transformed in place
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+            float t = acc[g][j] * p.alpha;
+            if (p.bias && c0 + j < p.N) t += __ldg(p.bias + c0 + j);
+            if (!ROPE) {
+                if (p.act == 1) t = gelu_erf(t);
+                else if (p.act == 2) t = fmaxf(t, 0.f);
+            }
+            v[j] = t;
+        }
+        if (ROPE && c0 < p.rope_ndst * p.rope_C) {
+            // this thread holds dims [d0, d0+32) of one head of token `row`: one RoPE axis (y: d0 = 0, x: d0 = 32),
+            // pairs (i, i+16) -- blocks.py:101-103 / pos_embed.py:129-159, fused with the head split
+            const int sec = c0 / p.rope_C, cc = c0 - sec * p.rope_C;
+            const int hh = cc >> 6, axis = (cc >> 5) & 1;
+            long long pz = __ldg(p.rope_pos + row * 2 + axis);
+            pz = pz < 0 ? 0 : (pz >= p.rope_npos ? p.rope_npos - 1 : pz);
+            const float4* tb = reinterpret_cast<const float4*>(p.rope_table + pz * 32);
+#pragma unroll
+            for (int i4 = 0; i4 < 8; ++i4) {
+                const float4 cs = __ldg(tb + i4);          // (cos, sin) of frequencies 2*i4 and 2*i4+1
+                const int i = 2 * i4;
+                const float u0 = v[i], w0 = v[i + 16], u1 = v[i + 1], w1 = v[i + 17];
+                v[i] = u0 * cs.x - w0 * cs.y;      v[i + 16] = w0 * cs.x + u0 * cs.y;
+                v[i + 1] = u1 * cs.z - w1 * cs.w;  v[i + 17] = w1 * cs.z + u1 * cs.w;
+            }
+            const long long bq = row / p.rope_ntok, nq = row - bq * p.rope_ntok;
+            const size_t off = (((size_t)bq * p.rope_heads + hh) * p.rope_ntok + nq) * 64 + axis * 32;
+            __nv_bfloat16* hp = p.rope_hi[sec] + off;
+            __nv_bfloat16* lp = p.rope_lo[sec] ? p.rope_lo[sec] + off : nullptr;
+#pragma unroll
+            for (int h8 = 0; h8 < 2; ++h8) {               // 16 values -> one 32-byte store of hi and of lo
+                uint32_t hw[8], lw[8];
+#pragma unroll
+                for (int k2 = 0; k2 < 8; ++k2) {
+                    const float a = v[16 * h8 + 2 * k2], b = v[16 * h8 + 2 * k2 + 1];
+                    const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
+                    const uint32_t hb = *reinterpret_cast<const uint32_t*>(&h2);
+                    const __nv_bfloat162 l2 = __floats2bfloat162_rn(a - __uint_as_float(hb << 16),
+                                                                    b - __uint_as_float(hb & 0xffff0000u));
+                    hw[k2] = hb;
+                    lw[k2] = *reinterpret_cast<const uint32_t*>(&l2);
+                }
+                st_v8_b32(hp + 16 * h8, hw);
+                if (lp) st_v8_b32(lp + 16 * h8, lw);
+            }
+            continue;
+        }
+        if (vec_ok && c0 + 32 <= p.N) {
+            if (!ROPE && p.residual) {
+                const float* rp = p.residual + rbase + (size_t)row * p.ldr + c0;
+#pragma unroll
+                for (int j8 = 0; j8 < 4; ++j8) {
+                    float rs[8];
+                    ld_v8_nc(rp + 8 * j8, rs);
+#pragma unroll
+                    for (int k2 = 0; k2 < 8; ++k2) v[8 * j8 + k2] += rs[k2];
+                }
+            }
+            if (p.D) {
+                float* dp = p.D + dbase + (size_t)row * p.ldd + c0;
+#pragma unroll
+                for (int j8 = 0; j8 < 4; ++j8) st_v8(dp + 8 * j8, v + 8 * j8);
+            }
+            if (!ROPE && p.Dhi) {
+                __nv_bfloat16* hp = p.Dhi + obase + (size_t)row * p.ldo + c0;
+                __nv_bfloat16* lp = p.Dlo ? p.Dlo + obase + (size_t)row * p.ldo + c0 : nullptr;
+#pragma unroll
+                for (int h8 = 0; h8 < 2; ++h8) {
+                    uint32_t hw[8], lw[8];
+#pragma unroll
+                    for (int k2 = 0; k2 < 8; ++k2) {
+                        float a = v[16 * h8 + 2 * k2], b = v[16 * h8 + 2 * k2 + 1];
+                        if (p.split_relu) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
+                        const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
+                        const uint32_t hb = *reinterpret_cast<const uint32_t*>(&h2);
+                        const __nv_bfloat162 l2 = __floats2bfloat162_rn(a - __uint_as_float(hb << 16),
+                                                                        b - __uint_as_float(hb & 0xffff0000u));
+                        hw[k2] = hb;
+                        lw[k2] = *reinterpret_cast<const uint32_t*>(&l2);
+                    }
+                    st_v8_b32(hp + 16 * h8, hw);
+                    if (lp) st_v8_b32(lp + 16 * h8, lw);
+                }
+            }
+        } else {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) {
+                if (c0 + j < p.N) {
+                    float t = v[j];
+                    if (!ROPE && p.residual) t += __ldg(p.residual + rbase + (size_t)row * p.ldr + c0 + j);
+                    if (p.D) p.D[dbase + (size_t)row * p.ldd + c0 + j] = t;
+                    if (!ROPE && p.Dhi) {
+                        const float ts = p.split_relu ? fmaxf(t, 0.f) : t;
+                        const __nv_bfloat16 h = __float2bfloat16_rn(ts);
+                        p.Dhi[obase + (size_t)row * p.ldo + c0 + j] = h;
+                        if (p.Dlo) p.Dlo[obase + (size_t)row * p.ldo + c0 + j] = __float2bfloat16_rn(ts - __bfloat162float(h));
+                    }
+                }
+            }
+        }
+    }
+}
+
 template <bool ROPE>
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_constant__ CUtensorMap mapAlo,
@@ -175,307 +228,144 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_constant
                const GemmParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    const int tiles_per_stage = p.nterms == 3 ? 4 : 2;
-    const uint32_t stage_bytes = tiles_per_stage * TILE_BYTES;
-    uint64_t* full_bar = (uint64_t*)(smem + (size_t)p.stages * stage_bytes);
-    uint64_t* empty_bar = full_bar + MAX_STAGES;
-    uint64_t* tmem_full_bar = empty_bar + MAX_STAGES;   // [2]
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;       // [2]
-    uint32_t* tmem_ptr = (uint32_t*)(tmem_empty_bar + 2);
+    const bool x3 = p.nterms == 3;
+    const uint32_t stage_bytes = (x3 ? 4 : 2) * TILE_BYTES;
+    uint64_t* full_bar = (uint64_t*)(smem + RING_BYTES);
+    uint64_t* empty_bar = full_bar + p.stages;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const bool conv = p.conv_wb > 0;
     const int tiles_m = conv ? p.conv_tiles_x * p.conv_tiles_y : (p.M + BM - 1) / BM;
     const int tiles_n = (p.N + BN - 1) / BN;
-    const int num_tiles = tiles_m * tiles_n * p.batch;
     const int num_kb = conv ? 9 * p.conv_chunks : (p.K + BK - 1) / BK;
+    const TileCoord tc = decode_tile(blockIdx.x, tiles_m, tiles_n);
+    const int m0 = tc.mt * BM, n0 = tc.nt * BN;
+    int x0 = 0, y0 = 0;
+    if (conv) { x0 = (tc.mt % p.conv_tiles_x) * p.conv_wb; y0 = (tc.mt / p.conv_tiles_x) * p.conv_hb; }
 
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&mapAhi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&mapBhi) : "memory");
-        if (p.nterms == 3) {
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&mapAlo) : "memory");
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&mapBlo) : "memory");
-        }
+    if (warp == 8 && lane == 0) {
+        prefetch_tensormap(&mapAhi);
+        prefetch_tensormap(&mapBhi);
+        if (x3) { prefetch_tensormap(&mapAlo); prefetch_tensormap(&mapBlo); }
+        for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar + s, 1); mbar_init(empty_bar + s, NCONSUMER / 32); }
+        mbar_init_fence();
     }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar + s, 1); mbar_init(empty_bar + s, 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(tmem_full_bar + b, 1); mbar_init(tmem_empty_bar + b, 8); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "n"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ===== TMA producer =====
-        if (elect_one()) {
-            uint32_t it = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-                const TileCoord tc = decode_tile(p, tile, tiles_m, tiles_n);
-                const int n0 = tc.nt * BN;
-                int m0 = tc.mt * BM, x0 = 0, y0 = 0;
-                if (conv) { x0 = (tc.mt % p.conv_tiles_x) * p.conv_wb; y0 = (tc.mt / p.conv_tiles_x) * p.conv_hb; }
-                for (int kb = 0; kb < num_kb; ++kb, ++it) {
-                    const int s = it % p.stages;
-                    const uint32_t ph = (it / p.stages) & 1;
-                    mbar_wait(empty_bar + s, ph ^ 1);
-                    uint8_t* st = smem + (size_t)s * stage_bytes;
-                    mbar_expect_tx(full_bar + s, stage_bytes);
-                    if (conv) {
-                        const int tap = kb / p.conv_chunks, ch = kb - tap * p.conv_chunks;
-                        const int cx = x0 + (tap % 3) - 1, cy = y0 + (tap / 3) - 1;
-                        tma_load_4d(st, &mapAhi, full_bar + s, ch * BK, cx, cy, tc.bz);
-                        if (p.nterms == 3) tma_load_4d(st + 2 * TILE_BYTES, &mapAlo, full_bar + s, ch * BK, cx, cy, tc.bz);
-                        tma_load_3d(st + TILE_BYTES, &mapBhi, full_bar + s, kb * BK, n0, 0);
-                        if (p.nterms == 3) tma_load_3d(st + 3 * TILE_BYTES, &mapBlo, full_bar + s, kb * BK, n0, 0);
-                    } else {
-                        tma_load_3d(st, &mapAhi, full_bar + s, kb * BK, m0, tc.bz);
-                        tma_load_3d(st + TILE_BYTES, &mapBhi, full_bar + s, kb * BK, n0, tc.bz);
-                        if (p.nterms == 3) {
-                            tma_load_3d(st + 2 * TILE_BYTES, &mapAlo, full_bar + s, kb * BK, m0, tc.bz);
-                            tma_load_3d(st + 3 * TILE_BYTES, &mapBlo, full_bar + s, kb * BK, n0, tc.bz);
-                        }
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        const uint32_t idesc = make_idesc();
-        uint32_t it = 0, lc = 0;   // lc counts (tile, K-chunk) units: each owns one TMEM accumulator buffer
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-            for (int kb0 = 0; kb0 < num_kb; kb0 += KCHUNK_KB, ++lc) {
-                const uint32_t buf = lc & 1;
-                mbar_wait(tmem_empty_bar + buf, ((lc >> 1) & 1) ^ 1);   // epilogue has drained this accumulator
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + buf * BN;
-                const int kb1 = min(kb0 + KCHUNK_KB, num_kb);
-                for (int kb = kb0; kb < kb1; ++kb, ++it) {
-                    const int s = it % p.stages;
-                    const uint32_t ph = (it / p.stages) & 1;
-                    mbar_wait(full_bar + s, ph);
-                    tc_fence_after();
-                    if (elect_one()) {
-                        const uint32_t st = smem_u32(smem + (size_t)s * stage_bytes);
-                        const uint64_t dAhi = make_smem_desc(st), dBhi = make_smem_desc(st + TILE_BYTES);
-                        const uint64_t dAlo = make_smem_desc(st + 2 * TILE_BYTES), dBlo = make_smem_desc(st + 3 * TILE_BYTES);
-#pragma unroll
-                        for (int k = 0; k < BK / UMMA_K; ++k) {
-                            const uint64_t adv = (uint64_t)((k * UMMA_K * 2) >> 4);  // +32 B per K step, in 16 B units
-                            tc_mma(tmem_d, dAhi + adv, dBhi + adv, idesc, ((kb - kb0) | k) ? 1u : 0u);
-                            if (p.nterms == 3) {
-                                tc_mma(tmem_d, dAhi + adv, dBlo + adv, idesc, 1u);
-                                tc_mma(tmem_d, dAlo + adv, dBhi + adv, idesc, 1u);
-                            }
-                        }
-                        tc_commit(empty_bar + s);                            // slot free once these MMAs retire
-                        if (kb == kb1 - 1) tc_commit(tmem_full_bar + buf);   // this chunk's partial sum is complete
-                    }
-                    __syncwarp();
-                }
-            }
-        }
-    } else if (warp >= 4) {
-        // ===== epilogue (8 warps): TMEM -> fp32 registers (K-chunk promotion) -> global =====
-        // warp e = warp-4: TMEM lane quarter q = e % 4 (hardware restriction), column half = e / 4 (64 columns each).
-        const int e = warp - 4;
-        const int q = e & 3, half = e >> 2;
-        uint32_t lc = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-            const TileCoord tc = decode_tile(p, tile, tiles_m, tiles_n);
-            const int n0 = tc.nt * BN + half * 64, m0 = tc.mt * BM, bz = tc.bz;
-            int x0 = 0, y0 = 0;
-            if (conv) { x0 = (tc.mt % p.conv_tiles_x) * p.conv_wb; y0 = (tc.mt / p.conv_tiles_x) * p.conv_hb; }
-            const int zo = bz / p.zdiv, zi = bz % p.zdiv;
-            const size_t dbase = (size_t)zo * p.sD2 + (size_t)zi * p.sD;
-            const size_t obase = (size_t)zo * p.sO2 + (size_t)zi * p.sO;
-            const size_t rbase = (size_t)zo * p.sR2 + (size_t)zi * p.sR;
-            // 256-bit accesses need 32 B alignment of every row segment
-            const bool vec_ok = (p.ldd % 8 == 0) && (p.ldr % 8 == 0) && (p.ldo % 16 == 0) &&
-                                (((uintptr_t)p.D | (uintptr_t)p.residual | (uintptr_t)p.Dhi | (uintptr_t)p.Dlo) % 32 == 0) &&
-                                ((dbase | rbase) % 8 == 0) && (obase % 16 == 0);
-            // The tensor core's fp32 accumulator truncates, so its error grows linearly with the length of the
-            // accumulation chain (measured: 1.2e-6 at K=1024, 2e-5 at K=16384).  Partial sums are therefore taken
-            // out of TMEM every KCHUNK_KB k-blocks and added here in round-to-nearest fp32 registers.
-            float acc[2][32];
-            for (int kb0 = 0; kb0 < num_kb; kb0 += KCHUNK_KB, ++lc) {
-                const uint32_t buf = lc & 1;
-                mbar_wait(tmem_full_bar + buf, (lc >> 1) & 1);
-                tc_fence_after();
-#pragma unroll
-                for (int g = 0; g < 2; ++g) {
-                    uint32_t r[32];
-                    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * BN + half * 64 + g * 32);
-                    asm volatile(
-                        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                        : "r"(taddr) : "memory");
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) acc[g][j] = kb0 == 0 ? __uint_as_float(r[j]) : acc[g][j] + __uint_as_float(r[j]);
-                }
-                tc_fence_before();
-                if (lane == 0) mbar_arrive(tmem_empty_bar + buf);   // hand the buffer back to the MMA warp
-            }
-            // lane == accumulator row: each thread owns 2 x 32 consecutive columns of one output row (two full 128 B
-            // lines), so every 128-bit load/store below moves whole sectors.
-            const int trow = q * 32 + lane;
-            long long row;
-            if (conv) {
-                const int yy = y0 + trow / p.conv_wb, xx = x0 + trow % p.conv_wb;
-                row = (yy < p.conv_H && xx < p.conv_W) ? (long long)yy * p.conv_W + xx : -1;
-            } else {
-                row = m0 + trow < p.M ? m0 + trow : -1;
-            }
-            if (row < 0) continue;
-#pragma unroll
-            for (int g = 0; g < 2; ++g) {
-                const int c0 = n0 + g * 32;
-                if (c0 >= p.N) continue;
-                float (&v)[32] = acc[g];      // finished accumulators are transformed in place
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    float t = acc[g][j] * p.alpha;
-                    if (p.bias && c0 + j < p.N) t += __ldg(p.bias + c0 + j);
-                    if (!ROPE) {
-                        if (p.act == 1) t = gelu_erf(t);
-                        else if (p.act == 2) t = fmaxf(t, 0.f);
-                    }
-                    v[j] = t;
-                }
-                if (ROPE && c0 < p.rope_ndst * p.rope_C) {
-                    // this thread holds dims [d0, d0+32) of one head of token `row`: one RoPE axis (y: d0 = 0, x: d0 = 32),
-                    // pairs (i, i+16) -- blocks.py:101-103 / pos_embed.py:129-159, fused with the head split
-                    const int sec = c0 / p.rope_C, cc = c0 - sec * p.rope_C;
-                    const int hh = cc >> 6, axis = (cc >> 5) & 1;
-                    long long pz = __ldg(p.rope_pos + row * 2 + axis);
-                    pz = pz < 0 ? 0 : (pz >= p.rope_npos ? p.rope_npos - 1 : pz);
-                    const float4* tb = reinterpret_cast<const float4*>(p.rope_table + pz * 32);
-#pragma unroll
-                    for (int i4 = 0; i4 < 8; ++i4) {
-                        const float4 cs = __ldg(tb + i4);          // (cos, sin) of frequencies 2*i4 and 2*i4+1
-                        const int i = 2 * i4;
-                        const float u0 = v[i], w0 = v[i + 16], u1 = v[i + 1], w1 = v[i + 17];
-                        v[i] = u0 * cs.x - w0 * cs.y;      v[i + 16] = w0 * cs.x + u0 * cs.y;
-                        v[i + 1] = u1 * cs.z - w1 * cs.w;  v[i + 17] = w1 * cs.z + u1 * cs.w;
-                    }
-                    const long long bq = row / p.rope_ntok, nq = row - bq * p.rope_ntok;
-                    const size_t off = (((size_t)bq * p.rope_heads + hh) * p.rope_ntok + nq) * 64 + axis * 32;
-                    __nv_bfloat16* hp = p.rope_hi[sec] + off;
-                    __nv_bfloat16* lp = p.rope_lo[sec] ? p.rope_lo[sec] + off : nullptr;
-#pragma unroll
-                    for (int h8 = 0; h8 < 2; ++h8) {               // 16 values -> one 32-byte store of hi and of lo
-                        uint32_t hw[8], lw[8];
-#pragma unroll
-                        for (int k2 = 0; k2 < 8; ++k2) {
-                            const float a = v[16 * h8 + 2 * k2], b = v[16 * h8 + 2 * k2 + 1];
-                            const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
-                            const uint32_t hb = *reinterpret_cast<const uint32_t*>(&h2);
-                            const __nv_bfloat162 l2 = __floats2bfloat162_rn(a - __uint_as_float(hb << 16),
-                                                                            b - __uint_as_float(hb & 0xffff0000u));
-                            hw[k2] = hb;
-                            lw[k2] = *reinterpret_cast<const uint32_t*>(&l2);
-                        }
-                        st_v8_b32(hp + 16 * h8, hw);
-                        if (lp) st_v8_b32(lp + 16 * h8, lw);
-                    }
-                    continue;
-                }
-                if (vec_ok && c0 + 32 <= p.N) {
-                    if (!ROPE && p.residual) {
-                        const float* rp = p.residual + rbase + (size_t)row * p.ldr + c0;
-#pragma unroll
-                        for (int j8 = 0; j8 < 4; ++j8) {
-                            float rs[8];
-                            ld_v8_nc(rp + 8 * j8, rs);
-#pragma unroll
-                            for (int k2 = 0; k2 < 8; ++k2) v[8 * j8 + k2] += rs[k2];
-                        }
-                    }
-                    if (p.D) {
-                        float* dp = p.D + dbase + (size_t)row * p.ldd + c0;
-#pragma unroll
-                        for (int j8 = 0; j8 < 4; ++j8) st_v8(dp + 8 * j8, v + 8 * j8);
-                    }
-                    if (!ROPE && p.Dhi) {
-                        __nv_bfloat16* hp = p.Dhi + obase + (size_t)row * p.ldo + c0;
-                        __nv_bfloat16* lp = p.Dlo ? p.Dlo + obase + (size_t)row * p.ldo + c0 : nullptr;
-#pragma unroll
-                        for (int h8 = 0; h8 < 2; ++h8) {
-                            uint32_t hw[8], lw[8];
-#pragma unroll
-                            for (int k2 = 0; k2 < 8; ++k2) {
-                                float a = v[16 * h8 + 2 * k2], b = v[16 * h8 + 2 * k2 + 1];
-                                if (p.split_relu) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
-                                const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
-                                const uint32_t hb = *reinterpret_cast<const uint32_t*>(&h2);
-                                const __nv_bfloat162 l2 = __floats2bfloat162_rn(a - __uint_as_float(hb << 16),
-                                                                                b - __uint_as_float(hb & 0xffff0000u));
-                                hw[k2] = hb;
-                                lw[k2] = *reinterpret_cast<const uint32_t*>(&l2);
-                            }
-                            st_v8_b32(hp + 16 * h8, hw);
-                            if (lp) st_v8_b32(lp + 16 * h8, lw);
-                        }
-                    }
+        if (lane == 0) {
+            for (int kb = 0; kb < num_kb; ++kb) {
+                const int s = kb % p.stages;
+                mbar_wait(empty_bar + s, ((kb / p.stages) & 1) ^ 1);
+                uint8_t* st = smem + (size_t)s * stage_bytes;
+                mbar_expect_tx(full_bar + s, stage_bytes);
+                if (conv) {
+                    const int tap = kb / p.conv_chunks, ch = kb - tap * p.conv_chunks;
+                    const int cx = x0 + (tap % 3) - 1, cy = y0 + (tap / 3) - 1;
+                    tma_load_4d(st, &mapAhi, full_bar + s, ch * BK, cx, cy, tc.bz);
+                    if (x3) tma_load_4d(st + 2 * TILE_BYTES, &mapAlo, full_bar + s, ch * BK, cx, cy, tc.bz);
+                    tma_load_3d(st + TILE_BYTES, &mapBhi, full_bar + s, kb * BK, n0, 0);
+                    if (x3) tma_load_3d(st + 3 * TILE_BYTES, &mapBlo, full_bar + s, kb * BK, n0, 0);
                 } else {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        if (c0 + j < p.N) {
-                            float t = v[j];
-                            if (!ROPE && p.residual) t += __ldg(p.residual + rbase + (size_t)row * p.ldr + c0 + j);
-                            if (p.D) p.D[dbase + (size_t)row * p.ldd + c0 + j] = t;
-                            if (!ROPE && p.Dhi) {
-                                const float ts = p.split_relu ? fmaxf(t, 0.f) : t;
-                                const __nv_bfloat16 h = __float2bfloat16_rn(ts);
-                                p.Dhi[obase + (size_t)row * p.ldo + c0 + j] = h;
-                                if (p.Dlo) p.Dlo[obase + (size_t)row * p.ldo + c0 + j] = __float2bfloat16_rn(ts - __bfloat162float(h));
-                            }
-                        }
+                    tma_load_3d(st, &mapAhi, full_bar + s, kb * BK, m0, tc.bz);
+                    tma_load_3d(st + TILE_BYTES, &mapBhi, full_bar + s, kb * BK, n0, tc.bz);
+                    if (x3) {
+                        tma_load_3d(st + 2 * TILE_BYTES, &mapAlo, full_bar + s, kb * BK, m0, tc.bz);
+                        tma_load_3d(st + 3 * TILE_BYTES, &mapBlo, full_bar + s, kb * BK, n0, tc.bz);
                     }
                 }
             }
         }
-        tc_fence_before();
+        return;
     }
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
+
+    // ===== consumers: warpgroup wg computes rows [64 wg, 64 wg + 64) of the tile =====
+    const int wg = warp >> 2;
+    float tot[64], acc[64];
+    for (int kb0 = 0; kb0 < num_kb; kb0 += KCHUNK_KB) {
+        const int kb1 = min(kb0 + KCHUNK_KB, num_kb);
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+        for (int kb = kb0; kb < kb1; ++kb) {
+            const int s = kb % p.stages;
+            mbar_wait(full_bar + s, (kb / p.stages) & 1);
+            const uint32_t st = smem_u32(smem + (size_t)s * stage_bytes);
+            const uint64_t dAhi = make_smem_desc(st + wg * (TILE_BYTES / 2)), dBhi = make_smem_desc(st + TILE_BYTES);
+            const uint64_t dAlo = make_smem_desc(st + 2 * TILE_BYTES + wg * (TILE_BYTES / 2));
+            const uint64_t dBlo = make_smem_desc(st + 3 * TILE_BYTES);
+            fence_regs(acc);
+            wgmma_fence();
+            // +32 B per K step, in 16 B descriptor units; the branch stays outside the MMA chains so that no register
+            // traffic separates them
+            if (x3) {
+#pragma unroll
+                for (int k = 0; k < BK / MMA_K; ++k) {
+                    const uint64_t adv = (uint64_t)((k * MMA_K * 2) >> 4);
+                    wgmma_m64n128k16_ss(acc, dAhi + adv, dBhi + adv);
+                    wgmma_m64n128k16_ss(acc, dAhi + adv, dBlo + adv);
+                    wgmma_m64n128k16_ss(acc, dAlo + adv, dBhi + adv);
+                }
+            } else {
+#pragma unroll
+                for (int k = 0; k < BK / MMA_K; ++k) {
+                    const uint64_t adv = (uint64_t)((k * MMA_K * 2) >> 4);
+                    wgmma_m64n128k16_ss(acc, dAhi + adv, dBhi + adv);
+                }
+            }
+            wgmma_commit();
+            wgmma_wait<1>();                       // the previous k-block's MMAs have retired: release its slot
+            fence_regs(acc);
+            if (kb > kb0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty_bar + (kb - 1) % p.stages);
+            }
+        }
+        wgmma_wait<0>();
+        fence_regs(acc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty_bar + (kb1 - 1) % p.stages);
+#pragma unroll
+        for (int i = 0; i < 64; ++i) tot[i] = kb0 == 0 ? acc[i] : tot[i] + acc[i];
     }
+
+    // ===== epilogue: restage through shared memory so that a thread owns 64 consecutive columns of one row =====
+    // Every load of this tile has landed and been consumed, so the ring is free once both warpgroups are past their MMAs.
+    float* stg = reinterpret_cast<float*>(smem);
+    asm volatile("bar.sync 1, %0;" ::"n"(NCONSUMER) : "memory");
+    {
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+        for (int i = 0; i < 64; i += 2) {
+            const int r = r0 + 8 * ((i >> 1) & 1), c = c0 + 8 * (i >> 2);
+            *reinterpret_cast<float2*>(stg + r * STG_LD + c) = make_float2(tot[i], tot[i + 1]);
+        }
+    }
+    asm volatile("bar.sync 1, %0;" ::"n"(NCONSUMER) : "memory");
+    const int trow = threadIdx.x & (BM - 1), half = threadIdx.x >> 7;
+    float out[2][32];
+#pragma unroll
+    for (int g = 0; g < 2; ++g)
+#pragma unroll
+        for (int j = 0; j < 32; j += 4) {
+            const float4 v = *reinterpret_cast<const float4*>(stg + trow * STG_LD + half * 64 + g * 32 + j);
+            out[g][j] = v.x; out[g][j + 1] = v.y; out[g][j + 2] = v.z; out[g][j + 3] = v.w;
+        }
+    const int zo = tc.bz / p.zdiv, zi = tc.bz % p.zdiv;
+    const size_t dbase = (size_t)zo * p.sD2 + (size_t)zi * p.sD;
+    const size_t obase = (size_t)zo * p.sO2 + (size_t)zi * p.sO;
+    const size_t rbase = (size_t)zo * p.sR2 + (size_t)zi * p.sR;
+    // 256-bit row segments need 32 B alignment
+    const bool vec_ok = (p.ldd % 8 == 0) && (p.ldr % 8 == 0) && (p.ldo % 16 == 0) &&
+                        (((uintptr_t)p.D | (uintptr_t)p.residual | (uintptr_t)p.Dhi | (uintptr_t)p.Dlo) % 32 == 0) &&
+                        ((dbase | rbase) % 8 == 0) && (obase % 16 == 0);
+    store_row<ROPE>(p, out, trow, conv, x0, y0, m0, n0 + half * 64, dbase, obase, rbase, vec_ok);
 }
 
-// ---- host side: TMA descriptors through the driver entry point (no libcuda link dependency) ----
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = (EncodeTiledFn)p;
-    }
-    return fn;
-}
-
+// ---- host side ----
 int encode(CUtensorMap* map, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
            const cuuint32_t* box, const char* what) {
-    EncodeTiledFn fn = get_encode_fn();
+    hopper::EncodeTiledFn fn = hopper::get_encode_fn();
     if (!fn) { adb_set_error_msg("cuTensorMapEncodeTiled driver entry point unavailable"); return ADB_ERR_CUDA; }
     cuuint32_t estr[4] = {1, 1, 1, 1};
     CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), dims, strides, box, estr,
@@ -510,21 +400,19 @@ int make_map_nhwc(CUtensorMap* map, const void* ptr, int B, int H, int W, int C,
 
 int launch(const CUtensorMap& mAhi, const CUtensorMap& mAlo, const CUtensorMap& mBhi, const CUtensorMap& mBlo,
            GemmParams& p, long long num_tiles, cudaStream_t stream) {
-    p.stages = p.nterms == 3 ? 3 : 6;
-    const size_t smem = (size_t)p.stages * (p.nterms == 3 ? 4 : 2) * TILE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+    ADB_REQUIRE(num_tiles < 2147483647LL, "adb_gemm_bf16: too many output tiles");
+    p.stages = RING_BYTES / ((p.nterms == 3 ? 4 : 2) * TILE_BYTES);
     static AdbDeviceOnce once;
-    int num_sms = 0;
     {
         const int rc = once.ensure([]() -> int {
-            ADB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-            ADB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+            ADB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+            ADB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
             return ADB_OK;
-        }, &num_sms);
+        });
         if (rc != ADB_OK) return rc;
     }
-    const int grid = (int)(num_tiles < num_sms ? num_tiles : num_sms);
-    if (p.rope_ndst > 0) gemm_tc_kernel<true><<<grid, NTHREADS, smem, stream>>>(mAhi, mAlo, mBhi, mBlo, p);
-    else gemm_tc_kernel<false><<<grid, NTHREADS, smem, stream>>>(mAhi, mAlo, mBhi, mBlo, p);
+    if (p.rope_ndst > 0) gemm_tc_kernel<true><<<(unsigned)num_tiles, NTHREADS, SMEM_BYTES, stream>>>(mAhi, mAlo, mBhi, mBlo, p);
+    else gemm_tc_kernel<false><<<(unsigned)num_tiles, NTHREADS, SMEM_BYTES, stream>>>(mAhi, mAlo, mBhi, mBlo, p);
     ADB_CHECK_LAUNCH("gemm_tc_kernel");
     return ADB_OK;
 }

@@ -438,9 +438,9 @@ ADB_API int adb_gauss_newton(int mode, int n_poses, int n_pts, int n_edges, floa
     int* it_p = state_out, *done_p = state_out + 1, *ok_p = state_out + 3;
     float* delta_p = (float*)(state_out + 2);
     p.Kdev = K4;
-    // enough CTAs to fill the GPU: the reference launches one 256-thread CTA per edge (128 edges = 128 CTAs on 148 SMs);
-    // here every edge's points are split so that about 8 CTAs per SM are in flight
-    int n_split = (148 * 8 + n_edges - 1) / n_edges;
+    // enough CTAs to fill the GPU: the reference launches one 256-thread CTA per edge (128 edges = 128 CTAs on 132 SMs);
+    // here every edge's points are split so that about 8 CTAs per SM of an H100 are in flight
+    int n_split = (132 * 8 + n_edges - 1) / n_edges;
     const int max_split = (n_pts + 4 * GN_THREADS - 1) / (4 * GN_THREADS);
     if (n_split > max_split) n_split = max_split;
     if (n_split < 1) n_split = 1;

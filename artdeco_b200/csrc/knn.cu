@@ -258,7 +258,7 @@ knn_query_kernel(long long P, long long Q, int K, const Grid* __restrict__ gp, c
 
 int build_grid(long long P, const float* points, const Ws& w, cudaStream_t stream) {
     bbox_init_kernel<<<1, 32, 0, stream>>>(w.bbox);
-    const int blocks = (int)((P + 255) / 256 < 148 * 8 ? (P + 255) / 256 : 148 * 8);
+    const int blocks = (int)((P + 255) / 256 < 132 * 8 ? (P + 255) / 256 : 132 * 8);
     bbox_kernel<<<blocks, 256, 0, stream>>>(P, points, w.bbox);
     grid_setup_kernel<<<1, 1, 0, stream>>>(P, w.bbox, w.grid);
     cell_id_kernel<<<adb_cdiv(P, 256), 256, 0, stream>>>(P, points, w.grid, w.keys_a, w.vals_a);

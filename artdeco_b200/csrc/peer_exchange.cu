@@ -156,16 +156,15 @@ int fill_ptrs(PeerPtrs* pp, void* const* ptrs, int world) {
     return ADB_OK;
 }
 
-// CTAs per exchange kernel (ADB_PEER_CTAS, 1..2368; default: no cap below 16 CTAs per SM).  The kernels are NVLink-bound, and
-// the trade-off is measured but not yet tuned: with grids over every SM the exchange alone takes 0.25 ms on 2 GPUs and 0.34 ms
-// on 8, but on 8 GPUs the remote stores of all 148 SMs stall the backward kernels running beside the push (project_bwd_multi
-// 0.31 ms instead of 0.08); with 32 CTAs of 256 threads that contention cannot occur, but the copies lose memory parallelism
-// (0.59 ms alone on 2 GPUs).
+// CTAs per exchange kernel (ADB_PEER_CTAS, 1..2112; default: no cap below 16 CTAs per SM of an H100).  The kernels are
+// NVLink-bound: grids over every SM give the exchange the most memory parallelism, but their remote stores can stall the
+// backward kernels running beside the push on many GPUs; a small cap (e.g. 32 CTAs) avoids that contention at the cost of
+// slower copies.  Not tuned on H100.
 int peer_ctas() {
     static int n = [] {
         const char* e = getenv("ADB_PEER_CTAS");
-        const int v = e ? atoi(e) : 148 * 16;
-        return v < 1 ? 1 : (v > 148 * 16 ? 148 * 16 : v);
+        const int v = e ? atoi(e) : 132 * 16;
+        return v < 1 ? 1 : (v > 132 * 16 ? 132 * 16 : v);
     }();
     return n;
 }

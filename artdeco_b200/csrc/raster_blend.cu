@@ -55,9 +55,8 @@ __device__ __forceinline__ float rcp_approx(float x) {
 // Each thread issues ONE 48-byte cp.async.bulk (global -> shared, SASS UBLKCP) for the record of its list entry of the NEXT
 // batch; completion is tracked by an mbarrier per buffer (every thread arrives once; issuing threads add expect_tx 48).
 // The copy engine fills buffer (b+1)&1 while the warps evaluate batch b from buffer b&1, so the dependent-load latency of the
-// gather (vals[idx] -> splats[g]) no longer sits between two block barriers.  OPT-IN (ADB_BLEND_TMA=1): measured 5 % slower
-// than the synchronous staging on B200 — ncu shows both kernels issue-bound (72-80 % issue-slot utilisation, long_scoreboard
-// 0.6 cycles per issue), i.e. the latency this hides was already hidden by 3-4 resident CTAs per SM.
+// gather (vals[idx] -> splats[g]) no longer sits between two block barriers.  OPT-IN (ADB_BLEND_TMA=1): the blend kernels are
+// issue-bound with 3-4 resident CTAs per SM already hiding the gather latency, so the synchronous staging is the default.
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
@@ -597,10 +596,8 @@ static int blend_fwd_impl(bool legacy, int W, int H, int n_per_cam, const float*
     ADB_REQUIRE(W > 0 && H > 0 && n_per_cam >= 0, "adb_raster_blend_fwd: bad sizes");
     ADB_REQUIRE(tile_offsets && colors && alphas && last_ids, "adb_raster_blend_fwd: null pointer");
     dim3 grid(adb_cdiv(W, ADB_TILE), adb_cdiv(H, ADB_TILE));
-    // ADB_BLEND_TMA=1: double-buffered cp.async.bulk (TMA) staging.  Measured on B200 at the bench workload (gpurun_out ->
-    // profiles/r02_summary.md): 0.406 ms vs 0.387 ms for the synchronous LDG staging — the kernel is issue-bound with 4 CTAs/SM
-    // hiding the gather latency already, so the extra prescale pass and mbarrier waits cost more than the prefetch saves.
-    // Default: synchronous.
+    // ADB_BLEND_TMA=1: double-buffered cp.async.bulk (TMA) staging.  Default: synchronous LDG staging (the kernel is
+    // issue-bound with 4 CTAs/SM hiding the gather latency, so the extra prescale pass and mbarrier waits buy nothing).
     static const int tma = getenv("ADB_BLEND_TMA") ? atoi(getenv("ADB_BLEND_TMA")) : 0;
     if (legacy)
         blend_fwd_kernel<true, false><<<grid, BLOCK, 0, stream>>>(W, H, splats, vals_sorted, tile_offsets, max(n_per_cam, 1),
@@ -667,14 +664,14 @@ static int blend_bwd_impl(bool legacy, int W, int H, int n_per_cam, const float*
     if (n_per_cam == 0) return ADB_OK;
     ADB_REQUIRE(v_splats, "adb_raster_blend_bwd: null v_splats");
     dim3 grid(adb_cdiv(W, ADB_TILE), adb_cdiv(H, ADB_TILE));
-    // A/B switches: ADB_BWD_SLOTS=32 -> 32-slot deferred-reduction buffer (2 CTAs/SM; measured 0.75 vs 0.64 ms);
-    // ADB_BWD_OCC=3 -> 79 registers, 3 CTAs/SM instead of the default 64 registers, 4 CTAs/SM (12 B of spills; 0.630 vs 0.640 ms).
+    // A/B switches: ADB_BWD_SLOTS=32 -> 32-slot deferred-reduction buffer (2 CTAs/SM);
+    // ADB_BWD_OCC=3 -> 79 registers, 3 CTAs/SM instead of the default 64 registers, 4 CTAs/SM.
     static const int slots = getenv("ADB_BWD_SLOTS") ? atoi(getenv("ADB_BWD_SLOTS")) : 16;
     static const int occ = getenv("ADB_BWD_OCC") ? atoi(getenv("ADB_BWD_OCC")) : 4;
     int rc;
 #define ADB_BWD_ARGS grid, W, H, n_per_cam, splats, vals_sorted, tile_offsets, alphas, last_ids, v_colors, v_alphas, v_splats, hit_mask, stream
-    // ADB_BLEND_TMA=1: double-buffered cp.async.bulk staging (+13 KB of shared memory: 3 CTAs/SM instead of 4); measured
-    // 0.667 ms vs 0.629 ms for the default, so it stays opt-in (same reason as the forward kernel).
+    // ADB_BLEND_TMA=1: double-buffered cp.async.bulk staging (+13 KB of shared memory: 3 CTAs/SM instead of 4); opt-in for
+    // the same reason as the forward kernel.
     static const int tma = getenv("ADB_BLEND_TMA") ? atoi(getenv("ADB_BLEND_TMA")) : 0;
     if (legacy) rc = launch_bwd<true, 16, 3, false>(ADB_BWD_ARGS);
     else if (slots == 32) rc = launch_bwd<false, 32, 2, false>(ADB_BWD_ARGS);

@@ -172,8 +172,8 @@ ADB_API int adb_raster_tile_offsets(long long n_isect, const int64_t* keys_sorte
 //            warp shuffles, only the wider exchanges go through shared memory (global memory for tiles beyond 4096
 //            entries) — then keys = cam|tile|depth_bits and vals = cam*N + gaussian are written out.
 //
-// COPIES = 4 replicas of every tile counter (selected by CTA index) cut the same-address serialisation of the L2 atomics:
-// with one counter per tile the count kernel ran at 45 G atomics/s (profiles/r02_summary.md).
+// COPIES = 4 replicas of every tile counter (selected by CTA index) cut the same-address serialisation of the L2 atomics
+// that a single counter per tile suffers.
 //
 // Why the order equals the reference's stable radix sort of (tile, depth): the reference emits keys Gaussian-major, so
 // inside one (tile, depth) tie the stable sort leaves ascending Gaussian ids — exactly the ascending order of the

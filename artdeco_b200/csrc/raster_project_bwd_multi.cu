@@ -287,8 +287,7 @@ sh_bwd_multi_kernel(int N, int C, const float* __restrict__ means, const float* 
     }
     float gm[3] = {0.f, 0.f, 0.f};
     // software pipeline: the colour gradient of view c+1 is in flight while view c is expanded.  (A two-lanes-per-Gaussian
-    // split of the 16 coefficients was measured SLOWER on B200: 0.42 vs 0.29 ms for 8 views — the duplicated basis evaluation
-    // costs more than the halved register footprint buys.)
+    // split of the 16 coefficients duplicates the basis evaluation, which costs more than the halved register footprint buys.)
     float gn[3] = {0.f, 0.f, 0.f};
     if (in) {
         const float* gp = g_rgb + (size_t)i * 3;

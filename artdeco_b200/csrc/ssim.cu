@@ -1,4 +1,4 @@
-// Fused differentiable SSIM (11x11 separable Gaussian window, zero padding) for sm_100a.
+// Fused differentiable SSIM (11x11 separable Gaussian window, zero padding) for sm_90a.
 //
 // Replaces the reference's fused-ssim extension:
 //   Reconstruct/submodules/fused-ssim/ssim.cu:62   fusedssimCUDA
@@ -6,9 +6,9 @@
 //   Reconstruct/submodules/fused-ssim/ssim.cu:434  fusedssim (host)       -> adb_ssim_forward
 //   Reconstruct/submodules/fused-ssim/ssim.cu:480  fusedssim_backward     -> adb_ssim_backward
 //
-// Design differences (B200-first, not a translation):
+// Design differences (not a translation):
 //  * 32x32 output tile per CTA (halo read amplification 1.72x instead of 2.64x), one CTA per
-//    (tile, batch*channel) plane so the grid is ~3.1k CTAs at 1080p x 3ch (21 waves over 148 SMs).
+//    (tile, batch*channel) plane so the grid is ~3.1k CTAs at 1080p x 3ch (24 waves over 132 SMs).
 //  * no memsets: every output element is written exactly once by the kernel (the reference
 //    zero-fills four tensors first, ssim.cu:455-460).
 //  * optional fused mean: the per-CTA sum of the SSIM map is reduced in-kernel and added to a

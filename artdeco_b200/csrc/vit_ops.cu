@@ -271,7 +271,7 @@ im2col_patch_kernel(int B, int H, int W, const float* __restrict__ img, __nv_bfl
     }
 }
 
-inline int grid_for(long long n) { long long g = (n + 255) / 256; return (int)(g < 148LL * 32 ? g : 148LL * 32); }
+inline int grid_for(long long n) { long long g = (n + 255) / 256; return (int)(g < 132LL * 32 ? g : 132LL * 32); }
 
 }  // namespace
 

@@ -11,8 +11,8 @@ import torch
 from .model import AsymmetricMASt3R, forward_pair
 
 # Pairs per GPU per step of the MASt3R bench leg (bench.py) AND of the graph-replay parity test (tests/test_mast3r.py): the
-# benchmarked configuration is the tested one.  8 pairs per GPU = BASELINE config 5's 64 loop-closure pairs over 8 GPUs; measured
-# 100.4 pairs/s at B=8 vs 95.5 at B=4 on one B200 (better wave quantisation of the M = B*2048-row GEMMs).
+# benchmarked configuration is the tested one.  8 pairs per GPU = BASELINE config 5's 64 loop-closure pairs over 8 GPUs (and
+# larger batches quantise the M = B*2048-row GEMMs onto the SMs in fuller waves).
 BENCH_PAIRS_PER_GPU = 8
 
 

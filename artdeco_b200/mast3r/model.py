@@ -4,7 +4,7 @@ checkpoint ARTDECO loads (ViT-L encoder, 12+12 ViT-B decoder blocks, catmlp+dpt 
 ``state_dict`` key names, and the three internals ARTDECO actually drives — ``_encode_image``, ``_decoder``,
 ``_downstream_head`` (VSLAM/utils_mast3r.py:30-36,127,132,179) — plus ``forward``.
 
-Every dense contraction of the transformer and of the local-feature MLP runs on the tcgen05 GEMM
+Every dense contraction of the transformer and of the local-feature MLP runs on the wgmma GEMM
 (csrc/gemm_tc.cu) with fused bias/GELU/residual epilogues; LayerNorm, RoPE + head split, softmax and the patch
 im2col are hand-written companion kernels (csrc/vit_ops.cu).  ``precision``:
   "bf16x3" (default)  three-term split product, fp32-class accuracy (meets the 1e-4 pointmap tolerance)
@@ -310,7 +310,7 @@ class AsymmetricMASt3R:
             g2, _ = self._linear(ops.split(f2.reshape(B * N2, E), self.x3), "decoder_embed", B * N2)
             c1, c2 = g1.view(B, N1, Dd), g2.view(B, N2, Dd)
             # The two decoder sides of a layer only depend on the previous layer's pair, so they run concurrently on two
-            # CUDA streams (at batch 1 each side's GEMMs fill less than half of the 148 SMs on their own).
+            # CUDA streams (at batch 1 each side's GEMMs fill less than half of the 132 SMs on their own).
             s1 = torch.cuda.current_stream()
             s2 = self._side_stream(f1.device)
             for i in range(self.cfg["dec_depth"]):
@@ -331,7 +331,7 @@ class AsymmetricMASt3R:
         return tuple(out1), tuple(out2)
 
     # ---- DPT head (dust3r/heads/dpt_head.py:34-65, croco/models/dpt_block.py:79-218,356-410) ----------------
-    # All 3x3 / 1x1 convolutions and both ConvTranspose layers run on the tcgen05 kernel (implicit GEMM over NHWC
+    # All 3x3 / 1x1 convolutions and both ConvTranspose layers run on the wgmma kernel (implicit GEMM over NHWC
     # activations); only the bilinear x2 upsampling (align_corners=True) and pixel rearrangements stay in torch.
     def _c3(self, x: Split, B, H, W, name, **kw):
         w = self._w[name + ".weight"]

@@ -244,7 +244,7 @@ def set_attention_variant(variant: int) -> int:
 
 
 def attention(q: Split, k: Split, vt: Split, B: int, h: int, Nq: int, Nk: int, Nkpad: int, scale: float, x3=True) -> Split:
-    """Fused softmax(scale * q k^T) v on tcgen05 (S/P stay in tensor/shared memory).  q,k: [B,h,N,64]; vt: [B,h,64,Nkpad];
+    """Fused softmax(scale * q k^T) v on wgmma (S/P stay in registers).  q,k: [B,h,N,64]; vt: [B,h,64,Nkpad];
     returns the bf16 split of the head-merged output [B*Nq, h*64]."""
     dev = q.hi.device
     C = h * 64

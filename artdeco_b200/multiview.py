@@ -5,7 +5,7 @@ One step = forward + backward of every LOCAL view of the batch against the repli
 exchange, leaving on every rank the sum over ALL views of the per-view gradients (the step's semantics become "sum of C view
 losses"; the reference optimises one view per step, Reconstruct/scene/scene_models/h3dgsv3.py:406-464).
 
-B200 specifics:
+Design:
   * the whole local compute (projection -> tile-bucketed intersection -> blend fwd -> blend bwd, per view) has no host
     sync (intersection buffers are sized by a capacity measured once) and is captured in ONE CUDA graph;
   * gradients are produced by the multi-view backward kernels (parameters read once, gradients written once);
@@ -65,8 +65,8 @@ class MultiViewStep:
         self.use_graph = graph
         # overlap_views=True runs consecutive views on two CUDA streams (the latency-bound projection / atomics / sort stages of
         # one view could fill the gaps of the other's issue-bound blend kernels; both streams fork from / join the caller's, so
-        # the pair is capturable in one graph).  MEASURED on B200: 11.55 vs 10.99 ms per 8-view step — co-running blend kernels
-        # of two views cost more than the overlap wins — so it is off by default.
+        # the pair is capturable in one graph).  Off by default: co-running issue-bound blend kernels of two views compete for
+        # the same issue slots.
         self.overlap_views = overlap_views and self.C > 1
         self._side = torch.cuda.Stream(device=dev) if self.overlap_views else None
         self.graph = None

@@ -289,10 +289,9 @@ def make_exchange(n_gaussians: int, views_local: int, device, group=None, kind: 
       * "nccl" — ``parallel.MultiViewExchange``, the library collectives;
       * "peer" — ``PeerExchange``, this library's kernels over NVLink peer memory (falls back to "nccl", with a warning, when the
         ranks cannot map each other's memory).
-    Measured on B200s (profiles/r02_summary.md): the peer exchange alone is faster than the two NCCL collectives (0.25 vs 0.30 ms
-    on 2 GPUs, 0.34 vs 0.39 ms on 8), but inside the step it has not beaten them: on 8 GPUs its stores from every SM slow the
-    backward kernels running beside it (step 1.99 vs 1.71 ms), and capping its grids (``ADB_PEER_CTAS=32``) trades that for slower
-    copies (2 GPUs: 5.75 vs 5.52 ms per step).  Until the grid size is tuned the library collectives stay the default."""
+    The peer exchange's stores from every SM can slow the backward kernels running beside it, and capping its grids
+    (``ADB_PEER_CTAS=32``) trades that for slower copies; until the grid size is tuned on H100 the library collectives stay the
+    default."""
     import os
 
     from .parallel import MultiViewExchange

@@ -1,4 +1,4 @@
-"""Synthetic-stream harness for BASELINE config 3 ("PINGPONG stream end-to-end (Frontend+Backend+Mapping), 1xB200";
+"""Synthetic-stream harness for BASELINE config 3 ("PINGPONG stream end-to-end (Frontend+Backend+Mapping), 1 GPU";
 SURVEY.md §8d: "100 frames of mast3r_pair + raster_scene growth").  No dataset or checkpoint exists offline, so the stream is
 synthetic, but the KERNEL MIX and its contention for one GPU are the reference's (run.sh:15-17 runs Frontend, Backend and the
 mapper as processes sharing the device):

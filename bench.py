@@ -58,11 +58,12 @@ def _peaks():
     if os.path.exists(p):
         with open(p) as f:
             return json.load(f), True
-    return {"hbm_gbs": 6650.0, "bf16_tflops_sustained": 1400.0, "sm_max_mhz": 1965.0}, False
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16, 1980 MHz max SM clock
+    return {"hbm_gbs": 3350.0, "bf16_tflops_sustained": 989.0, "sm_max_mhz": 1980.0}, False
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     def __init__(self, index: int):
         self.f = tempfile.NamedTemporaryFile("w+", suffix=".csv", delete=False)
@@ -234,6 +235,32 @@ class Watchdog:
         self._t.cancel()
 
 
+DUMP_SAMPLE = 100_000     # Gaussians per dumped gradient: v_sh alone is 192 MB at 1M, the sample keeps the dump near 24 MB
+
+
+def dump_outputs(out_dir, grads):
+    """The per-Gaussian gradients the timed step hands its caller (v_means, v_quats, v_scales, v_opac, v_sh), on a fixed
+    seeded sample of Gaussians (rows listed in sample_index.npy), as float32 .npy files."""
+    os.makedirs(out_dir, exist_ok=True)
+    idx = np.sort(np.random.default_rng(1234).choice(N_GAUSS, DUMP_SAMPLE, replace=False))
+    sel = torch.from_numpy(idx).to(grads["v_sh"].device)
+    np.save(os.path.join(out_dir, "sample_index.npy"), idx.astype(np.float64))
+    for name in ("v_means", "v_quats", "v_scales", "v_opac", "v_sh"):
+        np.save(os.path.join(out_dir, f"{name}.npy"), grads[name].index_select(0, sel).float().cpu().numpy())
+    log(f"outputs of the last timed step written to {out_dir}")
+
+
+def dump_mast3r_outputs(out_dir, outs):
+    """The per-view head outputs of the last timed MASt3R step (pts3d, conf, desc, ...), first 8 pairs, every 4th pixel in
+    each direction, as float32 mast3r_view{1,2}_<name>.npy."""
+    os.makedirs(out_dir, exist_ok=True)
+    for v, r in enumerate(outs, 1):
+        for name, t in r.items():
+            if torch.is_tensor(t) and t.is_floating_point():
+                np.save(os.path.join(out_dir, f"mast3r_view{v}_{name}.npy"), t[:8, ::4, ::4].float().cpu().numpy())
+    log(f"MASt3R outputs of the last timed step written to {out_dir}")
+
+
 def timed(fn, steps, warmup, dev, world):
     """W warm-up calls, then K calls between CUDA events, barrier + synchronize on both sides, max over ranks."""
     import torch.distributed as dist
@@ -271,7 +298,7 @@ def event_ms(fn, reps, warmup=3):
     return a.elapsed_time(b) / reps
 
 
-def bench_mast3r(dev, world, rank, steps, warmup, want_baselines):
+def bench_mast3r(dev, world, rank, steps, warmup, want_baselines, dump_dir=None):
     """MASt3R pair inference (2x _encode_image + _decoder + 2x _downstream_head) at 512x512, B pairs per GPU per step;
     pairs are split across GPUs with no collective (SURVEY.md §8e)."""
     from artdeco_b200 import _lib
@@ -288,8 +315,10 @@ def bench_mast3r(dev, world, rank, steps, warmup, want_baselines):
 
     graphed = GraphedForwardPair(model, B, 512, 512)     # one CUDA graph replay per step (two streams)
 
+    last = {}
+
     def step():
-        graphed(d1, d2)
+        last["out"] = graphed(d1, d2)
 
     def e2e_step():
         r1, r2 = graphed(h1, h2)                          # H2D copies of both image batches from pinned host memory
@@ -298,8 +327,10 @@ def bench_mast3r(dev, world, rank, steps, warmup, want_baselines):
             o[..., 3].copy_(r["conf"], non_blocking=True)
 
     log("mast3r model resident; timing")
-    k = max(3, min(steps, 10))
+    k = max(1, steps)
     ms = timed(step, k, max(3, warmup), dev, world)
+    if dump_dir and rank == 0:
+        dump_mast3r_outputs(dump_dir, last["out"])
     ms_e2e = timed(e2e_step, k, 3, dev, world)
     # B = 1: the Frontend's per-frame latency (VSLAM/CameraTracker.py:59-61 runs one pair per tracked frame)
     graphed1 = GraphedForwardPair(model, 1, 512, 512)
@@ -320,8 +351,8 @@ def bench_mast3r(dev, world, rank, steps, warmup, want_baselines):
     gemm_ms = sum(tot.get(n, (0.0, 0))[0] for n in ("adb_gemm_bf16", "adb_gemm_bf16_rope", "adb_conv3x3_bf16", "adb_attention_bf16"))
     pairs_s = world * B / (ms * 1e-3)
     peaks, measured = _peaks()
-    peak_tf = float(peaks.get("bf16_tflops_sustained", 1400.0))
-    peak_src = "measured (MEASURED_PEAKS.json bf16_tflops_sustained)" if measured else "fallback (B200_PROFILING.md ~1.4 PFLOP/s sustained)"
+    peak_tf = float(peaks.get("bf16_tflops_sustained", 989.0))
+    peak_src = "measured (MEASURED_PEAKS.json bf16_tflops_sustained)" if measured else "fallback (H100 SXM data sheet, 989 TFLOP/s dense bf16)"
     algo_tf = MAST3R_FLOP_PER_PAIR * B / (gemm_ms * 1e-3) / 1e12          # over the GEMM kernels' own time
     traffic = None
     prof = os.path.join(ROOT, "profiles", "traffic.json")
@@ -334,12 +365,12 @@ def bench_mast3r(dev, world, rank, steps, warmup, want_baselines):
     res = {
         "metric": "MASt3R pairs/s @512^2", "value": pairs_s, "unit": "pairs/s", "ms_per_step": ms, "pairs_per_gpu_per_step": B,
         "b1_latency_ms": ms_b1, "b1_pairs_per_s": world / (ms_b1 * 1e-3),
-        "precision": "bf16x3 (3 tcgen05 MMAs per product: fp32-class accuracy, 1e-4 pointmap tolerance)",
+        "precision": "bf16x3 (3 wgmma MMAs per product: fp32-class accuracy, 1e-4 pointmap tolerance)",
         "e2e": {"value": world * B / (ms_e2e * 1e-3), "unit": "pairs/s", "ms_per_step": ms_e2e,
                 "h2d_bytes_per_step": 2 * h1.numel() * 4, "d2h_bytes_per_step": 2 * out_host[0].numel() * 4,
                 "what": "two image batches from pinned host memory -> forward_pair -> pts3d+conf of both views copied back"},
         "gpu_launches": launches,
-        "roofline": {"bound": "tensor", "kernel": "gemm_tc_kernel + attn_fused_kernel (tcgen05 GEMM / implicit-GEMM conv / fused attention)",
+        "roofline": {"bound": "tensor", "kernel": "gemm_tc_kernel + attn_fused_kernel (wgmma GEMM / implicit-GEMM conv / fused attention)",
                      "achieved": algo_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": algo_tf / peak_tf,
                      "tensor_work_achieved": 3 * algo_tf, "tensor_work_frac": 3 * algo_tf / peak_tf,
                      "peak_source": peak_src, "traffic": traffic, "kernel_ms_per_step": gemm_ms,
@@ -351,7 +382,7 @@ def bench_mast3r(dev, world, rank, steps, warmup, want_baselines):
     }
     if want_baselines and rank == 0:
         # the reference's own GPU mode on this box: torch eager fp32 with TF32 matmuls (croco.py:13 sets allow_tf32), same batch
-        log("mast3r: reference GPU mode (torch eager fp32+TF32 restatement) on the same B200")
+        log("mast3r: reference GPU mode (torch eager fp32+TF32 restatement) on the same GPU")
         try:
             from oracle import mast3r_torch as mt
             prev = torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32
@@ -506,6 +537,10 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-mast3r", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the config-3 stream and config-5 legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last step computed as DIR/<name>.npy (float32): the "
+                         "rasterizer gradients on a seeded Gaussian sample and the MASt3R head outputs on a pixel grid, "
+                         "so that two builds can be compared output for output")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -548,6 +583,8 @@ def main():
     sampler = ClockSampler(local_rank) if rank == 0 else None
     ms_step = timed(engine.step, args.steps, args.warmup, dev, world)
     n_isect_local = engine.check_overflow()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, engine.grads)
 
     # per-stage live timing + launch count over K more steps, eager (CUDA events on the launching stream)
     engine.use_graph = False
@@ -657,7 +694,7 @@ def main():
     gpix_e2e = N_VIEWS * P / (ms_e2e * 1e-3) / 1e9
     peaks, measured = _peaks()
     peak = float(peaks["hbm_gbs"])
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if measured else "fallback (B200_PROFILING.md 6.65 TB/s)"
+    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if measured else "fallback (H100 SXM data sheet, 3.35 TB/s)"
     I_mean = float(np.mean(n_isect_all))
     I_loc = float(np.mean(n_isect_local))
     # algorithmic bytes (SURVEY.md §8d): per view 568N + 112I + 68P; dominant kernel = blend_bwd: 44I + 44P per launch
@@ -671,10 +708,10 @@ def main():
     # secondary bound (SURVEY.md §7.4/§8d): FP32 issue.  No-cull model: 256 pixel-threads x I splats x (25 FLOP + 1 MUFU)
     # forward, 2.5x that backward, at 4 warp-instructions per clock per SM; the kernels beat it because warp-level culling
     # never evaluates most (pixel, splat) pairs.
-    sm_mhz = float(peaks.get("sm_max_mhz", 1965.0))
-    issue_rate = 148 * 4 * sm_mhz * 1e6                       # warp-instructions / s
+    sm_mhz = float(peaks.get("sm_max_mhz", 1980.0))
+    issue_rate = 132 * 4 * sm_mhz * 1e6                       # warp-instructions / s
     fwd_issue_ms = 8 * I_loc * 26 / issue_rate * 1e3
-    issue = {"model": "256 px x I x (25 FLOP + 1 MUFU) / 32 lanes at 148 SM x 4 issue/clk (no culling)", "sm_mhz": sm_mhz,
+    issue = {"model": "256 px x I x (25 FLOP + 1 MUFU) / 32 lanes at 132 SM x 4 issue/clk (no culling)", "sm_mhz": sm_mhz,
              "blend_fwd_bound_ms": fwd_issue_ms, "blend_bwd_bound_ms": 2.5 * fwd_issue_ms,
              "blend_fwd_measured_ms": stage_ms.get("blend_fwd"), "blend_bwd_measured_ms": stage_ms.get("blend_bwd")}
     roofline = {"bound": "hbm", "kernel": dom, "achieved": dom_gbs, "peak": peak, "unit": "GB/s",
@@ -723,7 +760,7 @@ def main():
             "config": {"workload": WORKLOAD, "n_gaussians": N_GAUSS, "width": W, "height": H, "n_views": N_VIEWS,
                        "views_per_gpu": Cl, "n_isect_per_view": n_isect_all, "n_isect_mean": I_mean, "sh_degree": 3, "eps2d": 0.01,
                        "l2": "working set per step (params 236 MB + per-view records/keys/accumulators ~150 MB x views + grads "
-                             "236 MB) exceeds the 126 MB L2; no explicit flush",
+                             "236 MB) exceeds the 50 MB L2; no explicit flush",
                        "parallelism": f"view-parallel dp{world}: 8-view batch split over ranks, one gradient exchange per step"
                                       + (" (all-gather 12 B/view colour grads + all-reduce [N,11], overlapped)" if world > 1 else ""),
                        "graph": "local compute of the value leg replayed as one CUDA graph (no host sync inside the step)"},
@@ -765,7 +802,7 @@ def main():
     if not args.no_mast3r:
         wd = Watchdog(limit, on_hang).start()
         mast3r = bench_mast3r(dev, world, rank, args.steps, args.warmup,
-                              want_baselines=(world == 1 and not args.no_cpu_baseline))
+                              want_baselines=(world == 1 and not args.no_cpu_baseline), dump_dir=args.dump_outputs)
         wd.cancel()
     clocks = sampler.stop() if sampler else None   # sampled across every timed GPU leg (raster, e2e, MASt3R)
     if rank != 0:

@@ -1,4 +1,4 @@
-/* artdeco_b200 — C ABI of the B200-native (sm_100a) kernels behind ARTDECO's hot-path operators.
+/* artdeco_b200 — C ABI of the H100-native (sm_90a) kernels behind ARTDECO's hot-path operators.
  *
  * Conventions
  *   - every pointer is a DEVICE pointer unless the comment says HOST; tensors are dense, row-major, fp32
@@ -265,7 +265,7 @@ int adb_knn_index(long long P, const float* points, int K, long long Q, const in
                   const unsigned char* candidate /*[P] or NULL*/, float* dists /*[Q*K]*/, int32_t* ids /*[Q*K]*/,
                   void* ws, size_t ws_bytes, adb_stream_t stream);
 
-/* ---- MASt3R: tensor-core GEMM (tcgen05 + TMA) and its companions ----
+/* ---- MASt3R: tensor-core GEMM (wgmma + TMA) and its companions ----
  * adb_gemm_bf16 replaces every nn.Linear / q@k^T / attn@v of the reference model
  *   (VSLAM/thirdparty/mast3r/dust3r/croco/models/blocks.py:58-112,140-169; dust3r/dust3r/patch_embed.py:19-29;
  *    mast3r/catmlp_dpt_head.py:67-69): D[z] = act(alpha * A[z] * B[z]^T + bias) + residual[z],
@@ -288,7 +288,7 @@ int adb_gemm_bf16(int batch, int M, int N, int K, const void* A_hi, const void* 
 int adb_conv3x3_bf16(int B, int H, int W, int Cin, int Cout, const void* x_hi, const void* x_lo, const void* w_hi,
                      const void* w_lo, const float* bias, const float* residual, float* D, void* D_hi, void* D_lo, int act,
                      int split_relu, adb_stream_t stream);
-/* adb_attention_bf16: fused softmax(scale * Q K^T) V with the score matrix resident in tensor memory; replaces the three
+/* adb_attention_bf16: fused softmax(scale * Q K^T) V with the score matrix held in registers; replaces the three
  *   materialised torch ops at croco/models/blocks.py:105-109 (self) and :162-166 (cross).  head_dim 64.
  *   Q [B*heads,Nq,64], K [B*heads,Nk,64], Vt [B*heads,64,Nkpad] bf16 splits; O bf16 split [B,Nq,heads*64]. */
 int adb_attention_bf16(int B, int heads, int Nq, int Nk, int Nkpad, const void* Q_hi, const void* Q_lo, const void* K_hi,

@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE ONLY.  Builds the REFERENCE's own CUDA extensions from the sources where they lie under
-/root/reference into oracle/_ref/ (git-ignored, travels to the GPU box with the snapshot), for sm_100:
+/root/reference into oracle/_ref/ (git-ignored, travels to the GPU box with the snapshot), for sm_90:
   fused_ssim_ref   <- Reconstruct/submodules/fused-ssim/{ssim.cu,ext.cpp}      (flags of its setup.py:13-23)
   simple_knn_ref   <- Reconstruct/submodules/simple-knn/{simple_knn.cu,spatial.cu,ext.cpp}
   mast3r_matching_ref <- VSLAM/backend/src/matching_kernels.cu + oracle/matching_bind.cpp (our binding; gn.cpp needs Eigen)
@@ -51,7 +51,7 @@ def build_all(verbose: bool = False) -> None:
         bdir = OUT / name
         bdir.mkdir(parents=True, exist_ok=True)
         cpp_extension.load(name=name, sources=[_src(s) for s in cfg["sources"]],
-                           extra_cuda_cflags=cfg["cuda_flags"] + ["-gencode", "arch=compute_100,code=sm_100"],
+                           extra_cuda_cflags=cfg["cuda_flags"] + ["-gencode", "arch=compute_90,code=sm_90"],
                            extra_cflags=["-O3"], build_directory=str(bdir), verbose=verbose, is_python_module=False)
         print(f"[build_ref] built {_so(name)}")
 

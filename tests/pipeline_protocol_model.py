@@ -1,21 +1,22 @@
-"""TEST INFRASTRUCTURE: an executable model of the synchronisation protocols of the two fused-attention kernels and the GEMM
-(artdeco_b200/csrc/attn_tc.cu), explored under random interleavings on the CPU.
+"""TEST INFRASTRUCTURE: an executable model of the synchronisation protocols of the fused-attention kernel (both variants,
+artdeco_b200/csrc/attn_tc.cu) and the GEMM (artdeco_b200/csrc/gemm_tc.cu), explored under random interleavings on the CPU.
 
 Why: the kernels are warp-specialised pipelines glued together by mbarriers whose waits see only the PARITY of a phase.
-A protocol in which a barrier can complete two phases before a waiter looks deadlocks on hardware (this happened once: the
-first tensor-memory-P version hung under CUDA-graph replay) and no amount of single-kernel testing reliably shows it.  The
+A protocol in which a barrier can complete two phases before a waiter looks deadlocks on hardware (an earlier version of the
+attention kernel hung under CUDA-graph replay this way) and no amount of single-kernel testing reliably shows it.  The
 model reproduces exactly that semantics:
 
   * ``Barrier``  arrival count, phase counter; ``wait(parity)`` passes iff the parity of the CURRENT (incomplete) phase
                  differs from the awaited one -- so a waiter that is two phases late blocks forever, as on the GPU;
   * TMA loads    complete asynchronously and out of order (an agent picks any in-flight load);
-  * tensor pipe  tcgen05.mma / tcgen05.commit execute strictly in issue order, asynchronously to the issuing thread;
-  * every agent (producer warps, MMA warp, softmax warps) is a generator that blocks on barrier waits; a seeded random
+  * wgmma        each consumer warp's wgmma groups read shared memory asynchronously, in issue order, and
+                 ``wgmma.wait_group N`` blocks until at most N of the warp's groups are still in flight;
+  * every agent (producer warps, consumer warps) is a generator that blocks on barrier waits; a seeded random
     scheduler picks which runnable agent advances.
 
-Besides deadlock the model checks the DATA hazards with explicit state machines for the K / V stages, the S/P tensor-memory
-buffers and the O accumulators (e.g. "P V of block j reads P of block j", "an S product never overwrites scores or P that
-have not been consumed", "Q is not replaced while score products that read it are in flight").
+Besides deadlock the model checks the DATA hazards with explicit state for the Q buffer and the K / V / GEMM ring stages:
+every read finds the load it expects, and no load overwrites a buffer before all eight consumer warps have read it (e.g.
+"Q is not replaced while score products of the current item still read it").
 
 The transcription follows the kernels line by line; the barrier names are the kernels' enum names.
 """
@@ -51,7 +52,7 @@ class Machine:
     def __init__(self, seed):
         self.rng = random.Random(seed)
         self.bars = {}
-        self.pipe = deque()       # ("mma", fn) | ("commit", barrier name)
+        self.pipes = {}           # per consumer warp: in-flight wgmma groups (fn), executed in issue order
         self.loads = []           # (fn, barrier name)
         self.agents = {}
 
@@ -65,6 +66,13 @@ class Machine:
         b = self.bars[name]
         return lambda: b.passed(parity)
 
+    def inflight_at_most(self, warp, n):   # wgmma.wait_group n
+        q = self.pipes.setdefault(warp, deque())
+        return lambda: len(q) <= n
+
+    def issue(self, warp, fn):               # wgmma.mma_async ... ; wgmma.commit_group
+        self.pipes.setdefault(warp, deque()).append(fn)
+
     def run(self, max_steps=2_000_000):
         blocked = {n: None for n in self.agents}
         gens = dict(self.agents)
@@ -77,8 +85,9 @@ class Machine:
             if steps > max_steps:
                 raise Hazard("no progress bound exceeded")
             choices = [("agent", n) for n in gens if n not in done and (blocked[n] is StopIteration or blocked[n]())]
-            if self.pipe:
-                choices.append(("pipe", None))
+            for w, q in self.pipes.items():
+                if q:
+                    choices.append(("pipe", w))
             for i in range(len(self.loads)):
                 choices.append(("load", i))
             if not choices:
@@ -89,11 +98,7 @@ class Machine:
                              ", ".join(f"{b.name}={b.phase}/{b.pending}" for b in self.bars.values()))
             kind, which = self.rng.choice(choices)
             if kind == "pipe":
-                op, arg = self.pipe.popleft()
-                if op == "mma":
-                    arg()
-                else:
-                    self.bars[arg].arrive()
+                self.pipes[which].popleft()()
             elif kind == "load":
                 fn, barname = self.loads.pop(which)
                 fn()
@@ -109,205 +114,54 @@ class Machine:
                     done.add(n)
 
 
+class Buffer:
+    """A shared-memory buffer filled by TMA and read by every consumer warp.  ``tag`` names the load it holds; ``load``
+    refuses to overwrite contents that some warp has not finished reading."""
+
+    def __init__(self, name, readers=8):
+        self.name, self.readers, self.tag, self.reads = name, readers, None, readers
+
+    def load(self, tag):
+        def f():
+            if self.reads < self.readers:
+                raise Hazard(f"{self.name} overwritten with load {tag} while {self.readers - self.reads} warps still "
+                             f"had to read load {self.tag}")
+            self.tag, self.reads = tag, 0
+        return f
+
+    def read(self, tag):
+        if self.tag != tag:
+            raise Hazard(f"{self.name}: a read expected load {tag}, found {self.tag}")
+
+    def done(self, tag):            # this warp's last read of the contents
+        self.read(tag)
+        self.reads += 1
+
+
 # =====================================================================================================================
-# Variant 1 (default): one query tile per CTA, attn_fused_kernel
+# attn_fused_kernel<TILES> (artdeco_b200/csrc/attn_tc.cu): warp 8 loads Q and the K blocks of both passes, warp 9 the V^T
+# blocks, warps 0..7 (two warpgroups) compute.  TILES = 1: one item per CTA; TILES = 2: persistent CTAs over n_items.
 # =====================================================================================================================
-def variant1(nb, seed, kst=3, vst=3, pfull_per_buffer=True):
-    """``pfull_per_buffer=False`` reproduces the first tensor-memory-P version (one P-full barrier per half), which the
-    model must reject."""
+def attention(nb, n_items, tiles, seed, kst, vst):
     M = Machine(seed)
-    M.bar("QFULL", 1)
+    M.bar("QFULL", 1); M.bar("QEMPTY", 8)
     for s in range(kst):
-        M.bar(f"KFULL{s}", 1); M.bar(f"KEMPTY{s}", 1)
+        M.bar(f"KFULL{s}", 1); M.bar(f"KEMPTY{s}", 8)
     for s in range(vst):
-        M.bar(f"VFULL{s}", 1); M.bar(f"VEMPTY{s}", 1)
-    for s in range(2):
-        M.bar(f"SFULL{s}", 1); M.bar(f"SEMPTY{s}", 9)
-        for c in range(2):
-            M.bar(f"PFULL{s}{c}" if pfull_per_buffer else f"PFULL{c}", 4)
-    M.bar("OFULL", 1)
-    pf = (lambda s, c: f"PFULL{s}{c}") if pfull_per_buffer else (lambda s, c: f"PFULL{c}")
+        M.bar(f"VFULL{s}", 1); M.bar(f"VEMPTY{s}", 8)
+    Q = Buffer("Q")
+    K = [Buffer(f"K stage {s}") for s in range(kst)]
+    V = [Buffer(f"V stage {s}") for s in range(vst)]
 
-    K = [None] * kst              # (it) held by the stage, None = free/consumed
-    V = [None] * vst
-    S = [dict(kind=None, blk=None, reads=0, p=[False, False]) for _ in range(2)]
-    st = dict(q=False, o_terms=0)
-
-    def k_loaded(s, it):
-        def f():
-            if K[s] is not None:
-                raise Hazard(f"K stage {s} overwritten while it still holds load {K[s]}")
-            K[s] = it
-        return f
-
-    def v_loaded(s, j):
-        def f():
-            if V[s] is not None:
-                raise Hazard(f"V stage {s} overwritten while it still holds block {V[s]}")
-            V[s] = j
-        return f
-
-    def producer_k():
-        M.loads.append((lambda: st.__setitem__("q", True), "QFULL"))
-        for it in range(2 * nb):
-            s = it % kst
-            yield M.wait(f"KEMPTY{s}", ((it // kst) & 1) ^ 1)
-            M.loads.append((k_loaded(s, it), f"KFULL{s}"))
-
-    def producer_v():
-        for j in range(nb):
-            s = j % vst
-            yield M.wait(f"VEMPTY{s}", ((j // vst) & 1) ^ 1)
-            M.loads.append((v_loaded(s, j), f"VFULL{s}"))
-
-    def s_mma(it, s, ks):
-        def f():
-            if not st["q"]:
-                raise Hazard("S product before Q arrived")
-            if K[ks] != it:
-                raise Hazard(f"S product {it} found K load {K[ks]} in stage {ks}")
-            b = S[s]
-            if b["kind"] == "scores" and b["reads"] < 8:
-                raise Hazard(f"S buffer {s} overwritten before its scores were read")
-            if b["kind"] == "p" and not b.get("consumed"):
-                raise Hazard(f"S buffer {s} overwritten before P V consumed P")
-            S[s] = dict(kind="scores", blk=it, reads=0, p=[False, False], consumed=False)
-        return f
-
-    def k_release(ks):
-        def f():
-            K[ks] = None
-        return f
-
-    def pv_mma(j, s, c, vs):
-        def f():
-            b = S[s]
-            if b["blk"] != nb + j or not b["p"][c]:
-                raise Hazard(f"P V of block {j} half {c} read buffer {s} holding {b['blk']} p={b['p']}")
-            if V[vs] != j:
-                raise Hazard(f"P V of block {j} found V block {V[vs]}")
-            st["o_terms"] += 1
-            if c == 1:
-                b["consumed"] = True
-                V[vs] = None
-        return f
-
-    def mma():
-        yield M.wait("QFULL", 0)
-
-        def issue_s(it, full):
-            s, ks = it & 1, it % kst
-            yield M.wait(f"KFULL{ks}", (it // kst) & 1)
-            yield M.wait(f"SEMPTY{s}", ((it >> 1) & 1) ^ 1)
-            M.pipe.append(("mma", s_mma(it, s, ks)))
-            M.pipe.append(("mma", k_release(ks)))
-            M.pipe.append(("commit", f"KEMPTY{ks}"))
-            M.pipe.append(("commit", f"SFULL{s}"))
-            if not full:
-                M.bars[f"SEMPTY{s}"].arrive()
-        for it in range(nb):
-            yield from issue_s(it, False)
-        yield from issue_s(nb, True)
-        for j in range(nb):
-            if j + 1 < nb:
-                yield from issue_s(nb + j + 1, True)
-            vs = j % vst
-            yield M.wait(f"VFULL{vs}", (j // vst) & 1)
-            s = (nb + j) & 1
-            for c in range(2):
-                yield M.wait(pf(s, c), ((j >> 1) & 1) if pfull_per_buffer else (j & 1))
-                M.pipe.append(("mma", pv_mma(j, s, c, vs)))
-                if c == 1:
-                    M.pipe.append(("commit", f"VEMPTY{vs}"))
-                    M.pipe.append(("commit", f"SEMPTY{s}"))
-                    if j == nb - 1:
-                        M.pipe.append(("commit", "OFULL"))
-
-    def softmax(half):
-        def g():
-            for it in range(nb):
-                s = it & 1
-                yield M.wait(f"SFULL{s}", (it >> 1) & 1)
-                if S[s]["blk"] != it or S[s]["kind"] != "scores":
-                    raise Hazard(f"pass-1 softmax read buffer {s} holding {S[s]['blk']} instead of {it}")
-                S[s]["reads"] += 1
-                M.bars[f"SEMPTY{s}"].arrive()
-            for j in range(nb):
-                it = nb + j
-                s = it & 1
-                yield M.wait(f"SFULL{s}", (it >> 1) & 1)
-                b = S[s]
-                if b["blk"] != it:
-                    raise Hazard(f"pass-2 softmax read buffer {s} holding {b['blk']} instead of {it}")
-                b["reads"] += 1
-                b["pcount"] = b.get("pcount", {0: 0, 1: 0})
-                b["pcount"][half] += 1
-                if b["pcount"][half] == 4:
-                    b["p"][half] = True
-                    b["kind"] = "p"
-                M.bars[f"SEMPTY{s}"].arrive()
-                M.bars[pf(s, half)].arrive()
-            yield M.wait("OFULL", 0)
-            if st["o_terms"] != 2 * nb:
-                raise Hazard("epilogue ran before every P V product retired")
-        return g
-
-    M.agents = {"tma_k": producer_k(), "tma_v": producer_v(), "mma": mma()}
-    for w in range(8):
-        M.agents[f"softmax{w}"] = softmax(w >> 2)()
-    return M
-
-
-# =====================================================================================================================
-# Variant 2 (opt-in): two query tiles per persistent CTA, attn_fused2_kernel
-# =====================================================================================================================
-def variant2(nb, n_items, seed, kst=3, vst=2):
-    M = Machine(seed)
-    M.bar("QFULL", 1); M.bar("QEMPTY", 1)
-    for s in range(kst):
-        M.bar(f"KFULL{s}", 1); M.bar(f"KEMPTY{s}", 1)
-    for s in range(vst):
-        M.bar(f"VFULL{s}", 1); M.bar(f"VEMPTY{s}", 1)
-    for x in range(2):
-        M.bar(f"SFULL{x}", 1); M.bar(f"SDONE{x}", 4)
-        M.bar(f"OFULL{x}", 1); M.bar(f"OEMPTY{x}", 4)
-
-    K = [None] * kst
-    V = [None] * vst
-    S = [dict(n=None, kind=None, reads=0, p=False, consumed=True) for _ in range(2)]
-    Q = dict(item=None, inflight=0)
-    O = [dict(item=None, terms=0, read=4) for _ in range(2)]
-
-    def q_loaded(wi):
-        def f():
-            if Q["inflight"]:
-                raise Hazard("Q replaced while score products that read it are in flight")
-            Q["item"] = wi
-        return f
-
-    def k_loaded(s, kc):
-        def f():
-            if K[s] is not None:
-                raise Hazard(f"K stage {s} overwritten while holding load {K[s]}")
-            K[s] = kc
-        return f
-
-    def v_loaded(s, vc):
-        def f():
-            if V[s] is not None:
-                raise Hazard(f"V stage {s} overwritten while holding block {V[s]}")
-            V[s] = vc
-        return f
-
-    def producer_k():
+    def producer_qk():
         kc = 0
         for wi in range(n_items):
             yield M.wait("QEMPTY", (wi & 1) ^ 1)
-            M.loads.append((q_loaded(wi), "QFULL"))
-            for _ in range(2 * nb):
+            M.loads.append((Q.load(wi), "QFULL"))
+            for _ in range(2 * nb):                          # pass 1 then pass 2
                 s = kc % kst
                 yield M.wait(f"KEMPTY{s}", ((kc // kst) & 1) ^ 1)
-                M.loads.append((k_loaded(s, kc), f"KFULL{s}"))
+                M.loads.append((K[s].load(kc), f"KFULL{s}"))
                 kc += 1
 
     def producer_v():
@@ -316,216 +170,104 @@ def variant2(nb, n_items, seed, kst=3, vst=2):
             for _ in range(nb):
                 s = vc % vst
                 yield M.wait(f"VEMPTY{s}", ((vc // vst) & 1) ^ 1)
-                M.loads.append((v_loaded(s, vc), f"VFULL{s}"))
+                M.loads.append((V[s].load(vc), f"VFULL{s}"))
                 vc += 1
 
-    def mma():
-        kc = vc = 0
-        sc = [0, 0]
-
-        def s_mma(x, n, kc_, wi):
+    def consumer(w):
+        def score(ks, kc, wi, last_q):                      # wgmma S = Q_t K^T; commit; wait_group 0
             def f():
-                if Q["item"] != wi:
-                    raise Hazard(f"S product of item {wi} read Q of item {Q['item']}")
-                if K[kc_ % kst] != kc_:
-                    raise Hazard(f"S product found K load {K[kc_ % kst]} instead of {kc_}")
-                b = S[x]
-                if b["kind"] == "scores" and b["reads"] < 4:
-                    raise Hazard(f"S_{x} overwritten before its scores were read")
-                if b["kind"] == "p" and not b["consumed"]:
-                    raise Hazard(f"S_{x} overwritten before P V consumed P")
-                S[x] = dict(n=n, kind="scores", reads=0, p=False, consumed=False)
-                Q["inflight"] -= 1
-            return f
+                (Q.done if last_q else Q.read)(wi)
+                K[ks].read(kc)
+            M.issue(w, f)
+            yield M.inflight_at_most(w, 0)
 
-        def issue_s(x, kc_, wi):
-            if sc[x] > 0:
-                yield M.wait(f"SDONE{x}", (sc[x] - 1) & 1)
-            Q["inflight"] += 1
-            M.pipe.append(("mma", s_mma(x, sc[x], kc_, wi)))
-            M.pipe.append(("commit", f"SFULL{x}"))
-            sc[x] += 1
-
-        def k_release(kc_):
-            def f():
-                K[kc_ % kst] = None
-            return f
-
-        def pv(x, n, vc_, wi, first, last):
-            def f():
-                b = S[x]
-                if b["n"] != n or not b["p"]:
-                    raise Hazard(f"P V_{x} #{n} read S_{x} holding #{b['n']} p={b['p']}")
-                if V[vc_ % vst] != vc_:
-                    raise Hazard(f"P V found V block {V[vc_ % vst]} instead of {vc_}")
-                o = O[x]
-                if first:
-                    if o["read"] < 4:
-                        raise Hazard(f"O_{x} re-initialised before the previous item's epilogue read it")
-                    O[x] = o = dict(item=wi, terms=0, read=0)
-                o["terms"] += 1
-                b["consumed"] = True
-            return f
-
-        def v_release(vc_):
-            def f():
-                V[vc_ % vst] = None
-            return f
-
-        for wi in range(n_items):
-            yield M.wait("QFULL", wi & 1)
-            for _ in range(nb):                                   # pass 1
-                ks = kc % kst
-                yield M.wait(f"KFULL{ks}", (kc // kst) & 1)
-                yield from issue_s(0, kc, wi)
-                yield from issue_s(1, kc, wi)
-                M.pipe.append(("mma", k_release(kc)))
-                M.pipe.append(("commit", f"KEMPTY{ks}"))
-                kc += 1
-            ks = kc % kst                                          # first block of pass 2
-            yield M.wait(f"KFULL{ks}", (kc // kst) & 1)
-            yield from issue_s(0, kc, wi)
-            yield from issue_s(1, kc, wi)
-            M.pipe.append(("mma", k_release(kc)))
-            M.pipe.append(("commit", f"KEMPTY{ks}"))
-            kc += 1
-            for j in range(nb):
-                vs = vc % vst
-                yield M.wait(f"VFULL{vs}", (vc // vst) & 1)
-                more = j + 1 < nb
-                ks = kc % kst
-                if more:
-                    yield M.wait(f"KFULL{ks}", (kc // kst) & 1)
-                for x in range(2):
-                    yield M.wait(f"SDONE{x}", (sc[x] - 1) & 1)
-                    if j == 0:
-                        yield M.wait(f"OEMPTY{x}", (wi & 1) ^ 1)
-                    M.pipe.append(("mma", pv(x, sc[x] - 1, vc, wi, j == 0, not more)))
-                    if x == 1:
-                        M.pipe.append(("mma", v_release(vc)))
-                        M.pipe.append(("commit", f"VEMPTY{vs}"))
-                    if not more:
-                        M.pipe.append(("commit", f"OFULL{x}"))
-                    if more:
-                        yield from issue_s(x, kc, wi)
-                if more:
-                    M.pipe.append(("mma", k_release(kc)))
-                    M.pipe.append(("commit", f"KEMPTY{ks}"))
-                    kc += 1
-                else:
-                    M.pipe.append(("commit", "QEMPTY"))
-                vc += 1
-
-    def softmax(x):
         def g():
-            n = 0
+            kc = vc = 0
             for wi in range(n_items):
-                for _ in range(nb):
-                    yield M.wait(f"SFULL{x}", n & 1)
-                    b = S[x]
-                    if b["n"] != n or b["kind"] != "scores":
-                        raise Hazard(f"pass-1 softmax of tile {x} expected S #{n}, found #{b['n']} ({b['kind']})")
-                    b["reads"] += 1
-                    M.bars[f"SDONE{x}"].arrive()
-                    n += 1
-                for _ in range(nb):
-                    yield M.wait(f"SFULL{x}", n & 1)
-                    b = S[x]
-                    if b["n"] != n:
-                        raise Hazard(f"pass-2 softmax of tile {x} expected S #{n}, found #{b['n']}")
-                    b["reads"] += 1
-                    if b["reads"] == 4:
-                        b["kind"], b["p"] = "p", True
-                    M.bars[f"SDONE{x}"].arrive()
-                    n += 1
-                yield M.wait(f"OFULL{x}", wi & 1)
-                o = O[x]
-                if o["item"] != wi or o["terms"] != nb:
-                    raise Hazard(f"epilogue of item {wi} tile {x} saw O of item {o['item']} with {o['terms']}/{nb} terms")
-                o["read"] += 1
-                M.bars[f"OEMPTY{x}"].arrive()
+                yield M.wait("QFULL", wi & 1)
+                for _ in range(nb):                          # pass 1
+                    ks = kc % kst
+                    yield M.wait(f"KFULL{ks}", (kc // kst) & 1)
+                    for _ in range(tiles):
+                        yield from score(ks, kc, wi, False)
+                    K[ks].done(kc)
+                    M.bars[f"KEMPTY{ks}"].arrive()
+                    kc += 1
+                for j in range(nb):                          # pass 2
+                    ks, vs = kc % kst, vc % vst
+                    yield M.wait(f"KFULL{ks}", (kc // kst) & 1)
+                    yield M.wait(f"VFULL{vs}", (vc // vst) & 1)
+                    for t in range(tiles):
+                        last = t == tiles - 1 and j == nb - 1
+                        yield from score(ks, kc, wi, last)
+                        if last:
+                            M.bars["QEMPTY"].arrive()
+                        M.issue(w, (lambda vs_, vc_: lambda: V[vs_].read(vc_))(vs, vc))     # wgmma O += P V
+                        yield M.inflight_at_most(w, 0)
+                    K[ks].done(kc)
+                    V[vs].done(vc)
+                    M.bars[f"KEMPTY{ks}"].arrive()
+                    M.bars[f"VEMPTY{vs}"].arrive()
+                    kc += 1
+                    vc += 1
         return g
 
-    M.agents = {"tma_k": producer_k(), "tma_v": producer_v(), "mma": mma()}
+    M.agents = {"tma_qk": producer_qk(), "tma_v": producer_v()}
     for w in range(8):
-        M.agents[f"softmax{w}"] = softmax(w >> 2)()
+        M.agents[f"consumer{w}"] = consumer(w)()
     return M
 
 
+def variant1(nb, seed, kst=3, vst=3):
+    """One 128-query tile per CTA, one work item."""
+    return attention(nb, 1, 1, seed, kst, vst)
+
+
+def variant2(nb, n_items, seed, kst=3, vst=2):
+    """Two query tiles per persistent CTA, n_items work items."""
+    return attention(nb, n_items, 2, seed, kst, vst)
+
+
 # =====================================================================================================================
-# The persistent tcgen05 GEMM (artdeco_b200/csrc/gemm_tc.cu): TMA ring + double-buffered TMEM accumulator per (tile, K-chunk)
+# gemm_tc_kernel (artdeco_b200/csrc/gemm_tc.cu): one CTA per output tile; warp 8 fills the TMA ring, warps 0..7 (two
+# warpgroups) keep one k-block of wgmma in flight and release a ring slot one k-block late; the last slot of a K-chunk is
+# released after wait_group 0, before the partial sum is promoted.  n_tiles CTAs run side by side.
 # =====================================================================================================================
 def gemm(n_tiles, num_kb, seed, stages=3, kchunk=8):
     M = Machine(seed)
-    for s in range(stages):
-        M.bar(f"full{s}", 1); M.bar(f"empty{s}", 1)
-    for b in range(2):
-        M.bar(f"tmem_full{b}", 1); M.bar(f"tmem_empty{b}", 8)
-    stage = [None] * stages
-    acc = [dict(unit=None, kbs=0, reads=8) for _ in range(2)]        # unit = (tile, chunk index)
-    chunks = [(kb0, min(kb0 + kchunk, num_kb)) for kb0 in range(0, num_kb, kchunk)]
 
-    def loaded(s, it):
-        def f():
-            if stage[s] is not None:
-                raise Hazard(f"smem stage {s} overwritten while holding k-block load {stage[s]}")
-            stage[s] = it
-        return f
+    def cta(c):
+        for s in range(stages):
+            M.bar(f"full{c}.{s}", 1); M.bar(f"empty{c}.{s}", 8)
+        ring = [Buffer(f"CTA {c} stage {s}") for s in range(stages)]
 
-    def producer():
-        it = 0
-        for _ in range(n_tiles):
-            for _ in range(num_kb):
-                s = it % stages
-                yield M.wait(f"empty{s}", ((it // stages) & 1) ^ 1)
-                M.loads.append((loaded(s, it), f"full{s}"))
-                it += 1
+        def producer():
+            for kb in range(num_kb):
+                s = kb % stages
+                yield M.wait(f"empty{c}.{s}", ((kb // stages) & 1) ^ 1)
+                M.loads.append((ring[s].load(kb), f"full{c}.{s}"))
 
-    def mma_kb(s, it, buf, unit, first):
-        def f():
-            if stage[s] != it:
-                raise Hazard(f"MMA expected k-block load {it} in stage {s}, found {stage[s]}")
-            a = acc[buf]
-            if first:
-                if a["reads"] < 8:
-                    raise Hazard(f"accumulator {buf} re-initialised before the epilogue drained {a['unit']}")
-                acc[buf] = a = dict(unit=unit, kbs=0, reads=0)
-            elif a["unit"] != unit:
-                raise Hazard("accumulate into a buffer owned by another (tile, chunk)")
-            a["kbs"] += 1
-            stage[s] = None
-        return f
+        def consumer(w):
+            me = (c, w)
 
-    def mma():
-        it = lc = 0
-        for tile in range(n_tiles):
-            for ci, (kb0, kb1) in enumerate(chunks):
-                buf = lc & 1
-                yield M.wait(f"tmem_empty{buf}", ((lc >> 1) & 1) ^ 1)
-                for kb in range(kb0, kb1):
-                    s = it % stages
-                    yield M.wait(f"full{s}", (it // stages) & 1)
-                    M.pipe.append(("mma", mma_kb(s, it, buf, (tile, ci), kb == kb0)))
-                    M.pipe.append(("commit", f"empty{s}"))
-                    if kb == kb1 - 1:
-                        M.pipe.append(("commit", f"tmem_full{buf}"))
-                    it += 1
-                lc += 1
+            def g():
+                for kb0 in range(0, num_kb, kchunk):
+                    kb1 = min(kb0 + kchunk, num_kb)
+                    for kb in range(kb0, kb1):
+                        s = kb % stages
+                        yield M.wait(f"full{c}.{s}", (kb // stages) & 1)
+                        M.issue(me, (lambda s_, kb_: lambda: ring[s_].done(kb_))(s, kb))
+                        yield M.inflight_at_most(me, 1)
+                        if kb > kb0:
+                            M.bars[f"empty{c}.{(kb - 1) % stages}"].arrive()
+                    yield M.inflight_at_most(me, 0)
+                    M.bars[f"empty{c}.{(kb1 - 1) % stages}"].arrive()
+            return g
 
-    def epilogue():
-        lc = 0
-        for tile in range(n_tiles):
-            for ci, (kb0, kb1) in enumerate(chunks):
-                buf = lc & 1
-                yield M.wait(f"tmem_full{buf}", (lc >> 1) & 1)
-                a = acc[buf]
-                if a["unit"] != (tile, ci) or a["kbs"] != kb1 - kb0:
-                    raise Hazard(f"epilogue of {(tile, ci)} read accumulator of {a['unit']} with {a['kbs']} k-blocks")
-                a["reads"] += 1
-                M.bars[f"tmem_empty{buf}"].arrive()
-                lc += 1
+        M.agents[f"tma{c}"] = producer()
+        for w in range(8):
+            M.agents[f"consumer{c}.{w}"] = consumer(w)()
 
-    M.agents = {"tma": producer(), "mma": mma()}
-    for w in range(8):
-        M.agents[f"epi{w}"] = epilogue()
+    for c in range(n_tiles):
+        cta(c)
     return M

@@ -231,7 +231,7 @@ def _ref_ext(name):
 @pytest.mark.gpu
 @pytest.mark.parametrize("P", [5000, 200_000])
 def test_distcuda2_bit_identical_to_the_reference_build(cuda, P):
-    """oracle/_ref/simple_knn_ref.so is the reference's OWN simple_knn.cu compiled for sm_100 (oracle/build_ref.py)."""
+    """oracle/_ref/simple_knn_ref.so is the reference's OWN simple_knn.cu compiled for sm_90 (oracle/build_ref.py)."""
     ref = _ref_ext("simple_knn_ref")
     from artdeco_b200.knn import distCUDA2, distIndex2
     pts = synthetic.raster_scene(P, seed=2)["means"].to(cuda)

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM + ViT companion kernels against plain PyTorch fp64 references (floating-point kernels: the torch
+"""wgmma GEMM + ViT companion kernels against plain PyTorch fp64 references (floating-point kernels: the torch
 reference is the oracle here, per the tier rules)."""
 import pytest
 import torch

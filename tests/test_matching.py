@@ -99,7 +99,7 @@ def test_refine_matches_bit_exact_vs_oracle(cuda, F):
 
 @pytest.mark.gpu
 def test_matches_the_reference_cuda_build(cuda):
-    """The reference's own matching_kernels.cu (built for sm_100 with its --use_fast_math flags) on the same inputs."""
+    """The reference's own matching_kernels.cu (built for sm_90 with its --use_fast_math flags) on the same inputs."""
     from oracle import build_ref
     try:
         ref = build_ref.load("mast3r_matching_ref")

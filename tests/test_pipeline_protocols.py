@@ -1,6 +1,6 @@
-"""Random-interleaving exploration of the fused-attention kernels' mbarrier protocols (tests/pipeline_protocol_model.py).
-CPU only.  The shipped protocols must run to completion with every data-hazard check silent under thousands of schedules;
-the protocol of the first tensor-memory-P version (one P-full barrier per half) must be caught."""
+"""Random-interleaving exploration of the mbarrier protocols of the fused-attention kernel and the GEMM
+(tests/pipeline_protocol_model.py).  CPU only.  The shipped protocols must run to completion with every data-hazard check
+silent under thousands of schedules, and single-line mutations of them must be caught."""
 import pytest
 
 from pipeline_protocol_model import Hazard, variant1, variant2
@@ -16,18 +16,6 @@ def test_variant1_protocol_has_no_deadlock_or_hazard(nb):
 def test_variant1_protocol_other_ring_depths(kst, vst):
     for seed in range(150):
         variant1(5, seed, kst=kst, vst=vst).run()
-
-
-def test_model_catches_the_single_pfull_barrier_race():
-    """The version that hung under CUDA-graph replay: softmax of block j+1 can complete a second phase of the per-half
-    P-full barrier before the MMA warp has looked at the first; a parity wait cannot see two flips."""
-    caught = 0
-    for seed in range(400):
-        try:
-            variant1(6, seed, pfull_per_buffer=False).run()
-        except Hazard:
-            caught += 1
-    assert caught > 0, "the model no longer reproduces the known protocol bug"
 
 
 @pytest.mark.parametrize("nb,items", [(1, 1), (1, 3), (2, 2), (3, 3), (5, 2), (8, 2)])
@@ -61,17 +49,25 @@ def _mutant(old, new, which, args, seeds=120):
 
 
 @pytest.mark.parametrize("label,old,new,which,args", [
-    ("v2: S product not waiting for the previous scores/P to be consumed",
-     '            if sc[x] > 0:\n                yield M.wait(f"SDONE{x}", (sc[x] - 1) & 1)\n',
-     '            if False:\n                yield None\n', "variant2", (3, 3)),
-    ("v2: P V not waiting for P", '                    yield M.wait(f"SDONE{x}", (sc[x] - 1) & 1)\n                    if j == 0:',
-     '                    if j == 0:', "variant2", (3, 3)),
-    ("v2: Q replaced without waiting for the last score products", '            yield M.wait("QEMPTY", (wi & 1) ^ 1)\n',
-     '            pass\n', "variant2", (3, 3)),
-    ("v2: S-done barrier counting 3 of the 4 warps", 'M.bar(f"SFULL{x}", 1); M.bar(f"SDONE{x}", 4)',
-     'M.bar(f"SFULL{x}", 1); M.bar(f"SDONE{x}", 3)', "variant2", (3, 3)),
-    ("v1: S-empty barrier without the MMA warp's arrival", 'M.bar(f"SFULL{s}", 1); M.bar(f"SEMPTY{s}", 9)',
-     'M.bar(f"SFULL{s}", 1); M.bar(f"SEMPTY{s}", 8)', "variant1", (5,)),
+    ("attention: K-empty barrier counting 7 of the 8 consumer warps", 'M.bar(f"KFULL{s}", 1); M.bar(f"KEMPTY{s}", 8)',
+     'M.bar(f"KFULL{s}", 1); M.bar(f"KEMPTY{s}", 7)', "variant2", (3, 3)),
+    ("attention: V-empty barrier counting 7 of the 8 consumer warps", 'M.bar(f"VFULL{s}", 1); M.bar(f"VEMPTY{s}", 8)',
+     'M.bar(f"VFULL{s}", 1); M.bar(f"VEMPTY{s}", 7)', "variant1", (4,)),
+    ("attention: Q-empty arrival before the item's last score product",
+     '                        yield from score(ks, kc, wi, last)\n                        if last:\n'
+     '                            M.bars["QEMPTY"].arrive()\n',
+     '                        if last:\n                            M.bars["QEMPTY"].arrive()\n'
+     '                        yield from score(ks, kc, wi, last)\n', "variant2", (3, 3)),
+    ("attention: next Q loaded without waiting for Q-empty", '            yield M.wait("QEMPTY", (wi & 1) ^ 1)\n',
+     '            pass\n', "variant2", (2, 3)),
+    ("attention: pass 2 not waiting for the V block", '                    yield M.wait(f"VFULL{vs}", (vc // vst) & 1)\n',
+     '', "variant2", (3, 3)),
+    ("gemm: ring slot kb released instead of kb-1",
+     'M.bars[f"empty{c}.{(kb - 1) % stages}"].arrive()', 'M.bars[f"empty{c}.{kb % stages}"].arrive()', "gemm", (2, 12)),
+    ("gemm: slot released with two k-blocks of wgmma in flight", 'yield M.inflight_at_most(me, 1)',
+     'yield M.inflight_at_most(me, 2)', "gemm", (2, 12)),
+    ("gemm: empty barrier counting 7 of the 8 consumer warps", 'M.bar(f"full{c}.{s}", 1); M.bar(f"empty{c}.{s}", 8)',
+     'M.bar(f"full{c}.{s}", 1); M.bar(f"empty{c}.{s}", 7)', "gemm", (2, 12)),
 ])
 def test_model_is_sensitive_to_protocol_mutations(label, old, new, which, args):
     assert _mutant(old, new, which, args) > 0, label
@@ -79,7 +75,7 @@ def test_model_is_sensitive_to_protocol_mutations(label, old, new, which, args):
 
 @pytest.mark.parametrize("n_tiles,num_kb,stages", [(1, 1, 3), (3, 16, 3), (4, 9, 6), (2, 20, 3), (5, 3, 2)])
 def test_gemm_pipeline_protocol(n_tiles, num_kb, stages):
-    """gemm_tc_kernel: TMA ring, K-chunk promotion through the two TMEM accumulators, 8 epilogue warps."""
+    """gemm_tc_kernel: TMA ring, slots released one k-block late under wgmma_wait<1>, K-chunk promotion."""
     from pipeline_protocol_model import gemm
     for seed in range(150):
         gemm(n_tiles, num_kb, seed, stages=stages).run()

@@ -86,7 +86,7 @@ def test_ssim_rejects_cpu_tensors(cuda):
 
 @pytest.mark.gpu
 def test_matches_the_reference_cuda_build(cuda):
-    """oracle/_ref/fused_ssim_ref.so is the reference's OWN ssim.cu compiled for sm_100 (--use_fast_math, as its setup.py does)."""
+    """oracle/_ref/fused_ssim_ref.so is the reference's OWN ssim.cu compiled for sm_90 (--use_fast_math, as its setup.py does)."""
     from oracle import build_ref
     try:
         ref = build_ref.load("fused_ssim_ref")

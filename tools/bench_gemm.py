@@ -1,4 +1,4 @@
-"""Per-shape timing of the tcgen05 GEMM on the MASt3R shapes (CUDA events, 20 reps after 3 warm-ups)."""
+"""Per-shape timing of the wgmma GEMM on the MASt3R shapes (CUDA events, 20 reps after 3 warm-ups)."""
 import os
 import sys
 
