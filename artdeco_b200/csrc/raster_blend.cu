@@ -231,12 +231,19 @@ __device__ __forceinline__ int build_hit_list_from_mask(const unsigned char* __r
     return nhit;
 }
 
+// Record index of a sorted value: the multi-view entry points index the stacked [C,N,12] records with vals (= cam*N + g)
+// directly (wrap = 0); the single-view ones pass wrap = N, because their vals may carry a camera offset while `splats` holds
+// that one camera's records.
+__device__ __forceinline__ int record_index(int v, int wrap) { return wrap ? v % wrap : v; }
+
+// Views: blockIdx.z = view c.  tile_offsets [C][T+1] are absolute indices into vals / hit_mask; colors / alphas / last_ids /
+// main_ids are [C,H,W,...] stacks.
 // LEGACY = Inria conventions (ADB_CONV_INRIA): alpha <= 0.99, stop when T(1-alpha) < 1e-4 (strict), 4th channel
 // accumulates 1/z, and main_ids gets the Gaussian with the largest blending weight alpha*T per pixel (-1: none).
 template <bool LEGACY, bool ASYNC>
 __global__ void __launch_bounds__(BLOCK, 4)
 blend_fwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* __restrict__ vals,
-                 const int32_t* __restrict__ tile_offsets, int n_per_cam,
+                 const int32_t* __restrict__ tile_offsets, int wrap,
                  float* __restrict__ colors, float* __restrict__ alphas, int32_t* __restrict__ last_ids,
                  int32_t* __restrict__ main_ids, unsigned char* __restrict__ hit_mask) {
     constexpr float MAXA = LEGACY ? ADB_MAX_ALPHA_INRIA : ADB_MAX_ALPHA;
@@ -254,7 +261,9 @@ blend_fwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
     const bool inside = (i < H && j < W);
     const float px = (float)j + 0.5f, py = (float)i + 0.5f;
     const WarpRect rect{(float)x0 + 0.5f, (float)x0 + 7.5f, (float)y0 + 0.5f, (float)y0 + 3.5f};
-    const int start = tile_offsets[tile], end = tile_offsets[tile + 1];
+    const size_t view_pix = (size_t)blockIdx.z * H * W;
+    const int orow = blockIdx.z * (gridDim.x * gridDim.y + 1) + tile;
+    const int start = tile_offsets[orow], end = tile_offsets[orow + 1];
     if (tid < BLOCK / 4) sMask[tid] = 0u;
     // Writes the finished batch's warp masks to hit_mask[start + pb*BLOCK ...] and clears the table (one thread per word, so the
     // clear cannot race with the read; the barrier that follows orders it before the next batch's atomics).
@@ -283,7 +292,7 @@ blend_fwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
         __syncthreads();
         if (nb > 0) {       // prologue: batch 0 -> buffer 0
             const int idx0 = start + tid;
-            issue_record_copy(sRecBuf[0] + tid * 3, splats, idx0 < end ? vals[idx0] % n_per_cam : 0, idx0 < end, &sBar[0]);
+            issue_record_copy(sRecBuf[0] + tid * 3, splats, idx0 < end ? record_index(vals[idx0], wrap) : 0, idx0 < end, &sBar[0]);
         }
     }
 
@@ -304,14 +313,14 @@ blend_fwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
             if (b + 1 < nb) {                            // prefetch batch b+1 into the buffer batch b-1 has just released
                 const int idx1 = idx + BLOCK;
                 fence_proxy_async();
-                issue_record_copy(sRecBuf[(b + 1) & 1] + tid * 3, splats, idx1 < end ? vals[idx1] % n_per_cam : 0, idx1 < end,
+                issue_record_copy(sRecBuf[(b + 1) & 1] + tid * 3, splats, idx1 < end ? record_index(vals[idx1], wrap) : 0, idx1 < end,
                                   &sBar[(b + 1) & 1]);
             }
             mbar_wait(&sBar[b & 1], (b >> 1) & 1);
             if (idx < end) prescale_record<LEGACY>(sRec + tid * 3);
         } else {
             if (n_done >= BLOCK) break;
-            if (idx < end) stage_record<LEGACY>(sRec + tid * 3, splats, vals[idx] % n_per_cam);
+            if (idx < end) stage_record<LEGACY>(sRec + tid * 3, splats, record_index(vals[idx], wrap));
         }
         __syncthreads();
         pending = b;
@@ -360,11 +369,11 @@ blend_fwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
         flush_mask(pending);
     }
     if (inside) {
-        const size_t pix = (size_t)i * W + j;
+        const size_t pix = view_pix + (size_t)i * W + j;
         reinterpret_cast<float4*>(colors)[pix] = acc;
         alphas[pix] = 1.0f - T;
         last_ids[pix] = cur;
-        if (LEGACY && main_ids) main_ids[pix] = best_k >= 0 ? vals[best_k] % n_per_cam : -1;
+        if (LEGACY && main_ids) main_ids[pix] = best_k >= 0 ? record_index(vals[best_k], wrap) : -1;
     }
 }
 
@@ -396,7 +405,7 @@ struct BwdSmem {
 template <bool LEGACY, int S, int OCC, bool ASYNC>
 __global__ void __launch_bounds__(BLOCK, OCC)
 blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* __restrict__ vals,
-                 const int32_t* __restrict__ tile_offsets, int n_per_cam,
+                 const int32_t* __restrict__ tile_offsets, int wrap,
                  const float* __restrict__ alphas, const int32_t* __restrict__ last_ids,
                  const float* __restrict__ v_colors, const float* __restrict__ v_alphas,
                  float* __restrict__ v_splats, const unsigned char* __restrict__ hit_mask) {
@@ -422,10 +431,12 @@ blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
     const bool inside = (i < H && j < W);
     const float px = (float)j + 0.5f, py = (float)i + 0.5f;
     const WarpRect rect{(float)x0 + 0.5f, (float)x0 + 7.5f, (float)y0 + 0.5f, (float)y0 + 3.5f};
-    const int start = tile_offsets[tile], end = tile_offsets[tile + 1];
+    // view row of tile_offsets by a 32-bit index (a 64-bit pointer bump here costs the 64-register build one more spill slot)
+    const int orow = blockIdx.z * (gridDim.x * gridDim.y + 1) + tile;
+    const int start = tile_offsets[orow], end = tile_offsets[orow + 1];
     if (end <= start) return;
 
-    const size_t pix = (size_t)(inside ? i : 0) * W + (inside ? j : 0);
+    const size_t pix = (size_t)blockIdx.z * H * W + (size_t)(inside ? i : 0) * W + (inside ? j : 0);
     const float T_final = inside ? 1.0f - alphas[pix] : 1.0f;
     const int bin_final = inside ? last_ids[pix] : -1;
     const float4 vo = inside ? reinterpret_cast<const float4*>(v_colors)[pix] : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -460,7 +471,7 @@ blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
     if (ASYNC) {
         __syncthreads();
         const int idx0 = end - 1 - tid;                      // prologue: batch 0 -> buffer 0
-        const int g0 = idx0 >= start ? vals[idx0] % n_per_cam : 0;
+        const int g0 = idx0 >= start ? record_index(vals[idx0], wrap) : 0;
         if (idx0 >= start) sG[tid] = g0;
         issue_record_copy(sRec + tid * 3, splats, g0, idx0 >= start, &sBar[0]);
     }
@@ -477,7 +488,7 @@ blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
             if (b + 1 < nb) {                                // prefetch batch b+1 into the buffer batch b-1 has just released
                 const int nbuf = (b + 1) & 1;
                 const int idx1 = idx - BLOCK;
-                const int g1 = idx1 >= start ? vals[idx1] % n_per_cam : 0;
+                const int g1 = idx1 >= start ? record_index(vals[idx1], wrap) : 0;
                 if (idx1 >= start) reinterpret_cast<int*>(reinterpret_cast<unsigned char*>(sG0) + nbuf * L::G_BYTES)[tid] = g1;
                 fence_proxy_async();
                 issue_record_copy(reinterpret_cast<float4*>(reinterpret_cast<unsigned char*>(sRec0) + nbuf * L::REC_BYTES) + tid * 3,
@@ -486,7 +497,7 @@ blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
             mbar_wait(&sBar[b & 1], (b >> 1) & 1);
             if (idx >= start) prescale_record<LEGACY>(sRec + tid * 3);
         } else if (idx >= start) {
-            const int g = vals[idx] % n_per_cam;
+            const int g = record_index(vals[idx], wrap);
             sG[tid] = g;
             stage_record<LEGACY>(sRec + tid * 3, splats, g);
         }
@@ -590,34 +601,42 @@ blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
 
 }  // namespace
 
-static int blend_fwd_impl(bool legacy, int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
+// C views (gridDim.z); wrap: see record_index.
+static int blend_fwd_impl(bool legacy, int C, int W, int H, int wrap, const float* splats, const int32_t* vals_sorted,
                           const int32_t* tile_offsets, float* colors, float* alphas, int32_t* last_ids,
                           int32_t* main_ids, unsigned char* hit_mask, cudaStream_t stream) {
-    ADB_REQUIRE(W > 0 && H > 0 && n_per_cam >= 0, "adb_raster_blend_fwd: bad sizes");
-    ADB_REQUIRE(tile_offsets && colors && alphas && last_ids, "adb_raster_blend_fwd: null pointer");
-    dim3 grid(adb_cdiv(W, ADB_TILE), adb_cdiv(H, ADB_TILE));
+    dim3 grid(adb_cdiv(W, ADB_TILE), adb_cdiv(H, ADB_TILE), C);
     // ADB_BLEND_TMA=1: double-buffered cp.async.bulk (TMA) staging.  Default: synchronous LDG staging (the kernel is
     // issue-bound with 4 CTAs/SM hiding the gather latency, so the extra prescale pass and mbarrier waits buy nothing).
     static const int tma = getenv("ADB_BLEND_TMA") ? atoi(getenv("ADB_BLEND_TMA")) : 0;
     if (legacy)
-        blend_fwd_kernel<true, false><<<grid, BLOCK, 0, stream>>>(W, H, splats, vals_sorted, tile_offsets, max(n_per_cam, 1),
+        blend_fwd_kernel<true, false><<<grid, BLOCK, 0, stream>>>(W, H, splats, vals_sorted, tile_offsets, wrap,
                                                                  colors, alphas, last_ids, main_ids, hit_mask);
     else if (tma)
-        blend_fwd_kernel<false, true><<<grid, BLOCK, 0, stream>>>(W, H, splats, vals_sorted, tile_offsets, max(n_per_cam, 1),
+        blend_fwd_kernel<false, true><<<grid, BLOCK, 0, stream>>>(W, H, splats, vals_sorted, tile_offsets, wrap,
                                                                  colors, alphas, last_ids, nullptr, hit_mask);
     else
-        blend_fwd_kernel<false, false><<<grid, BLOCK, 0, stream>>>(W, H, splats, vals_sorted, tile_offsets, max(n_per_cam, 1),
+        blend_fwd_kernel<false, false><<<grid, BLOCK, 0, stream>>>(W, H, splats, vals_sorted, tile_offsets, wrap,
                                                                   colors, alphas, last_ids, nullptr, hit_mask);
     ADB_CHECK_LAUNCH("blend_fwd_kernel");
     return ADB_OK;
+}
+
+static int blend_fwd_single(bool legacy, int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
+                            const int32_t* tile_offsets, float* colors, float* alphas, int32_t* last_ids,
+                            int32_t* main_ids, unsigned char* hit_mask, cudaStream_t stream) {
+    ADB_REQUIRE(W > 0 && H > 0 && n_per_cam >= 0, "adb_raster_blend_fwd: bad sizes");
+    ADB_REQUIRE(tile_offsets && colors && alphas && last_ids, "adb_raster_blend_fwd: null pointer");
+    return blend_fwd_impl(legacy, 1, W, H, max(n_per_cam, 1), splats, vals_sorted, tile_offsets, colors, alphas, last_ids,
+                          main_ids, hit_mask, stream);
 }
 
 // `vals` are the sorted values (cam*N + gaussian); n_per_cam = N.  colors [H,W,4], alphas [H,W], last_ids [H,W].
 ADB_API int adb_raster_blend_fwd(int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
                                  const int32_t* tile_offsets, float* colors, float* alphas, int32_t* last_ids,
                                  cudaStream_t stream) {
-    return blend_fwd_impl(false, W, H, n_per_cam, splats, vals_sorted, tile_offsets, colors, alphas, last_ids, nullptr,
-                          nullptr, stream);
+    return blend_fwd_single(false, W, H, n_per_cam, splats, vals_sorted, tile_offsets, colors, alphas, last_ids, nullptr,
+                            nullptr, stream);
 }
 
 // Same, and hit_mask[k] (one byte per sorted intersection, k as in vals_sorted) receives the warps of entry k's tile whose 8x4
@@ -627,20 +646,34 @@ ADB_API int adb_raster_blend_fwd_hits(int W, int H, int n_per_cam, const float* 
                                       const int32_t* tile_offsets, float* colors, float* alphas, int32_t* last_ids,
                                       unsigned char* hit_mask, cudaStream_t stream) {
     ADB_REQUIRE(hit_mask, "adb_raster_blend_fwd_hits: null hit_mask");
-    return blend_fwd_impl(false, W, H, n_per_cam, splats, vals_sorted, tile_offsets, colors, alphas, last_ids, nullptr,
-                          hit_mask, stream);
+    return blend_fwd_single(false, W, H, n_per_cam, splats, vals_sorted, tile_offsets, colors, alphas, last_ids, nullptr,
+                            hit_mask, stream);
+}
+
+// C views in one launch (the multi-view batch): splats [C,N,12] indexed by vals_sorted (= c*N + gaussian) directly,
+// tile_offsets [C,T+1] absolute (adb_raster_tile_scan_multi), colors [C,H,W,4], alphas / last_ids [C,H,W]; hit_mask (may be
+// NULL) indexed like vals_sorted.  Per view the result of adb_raster_blend_fwd_hits on that view's records, bit for bit;
+// last_ids are absolute sorted indices.  N = 0 (no Gaussians: every tile is empty) writes empty images; splats may be NULL.
+ADB_API int adb_raster_blend_fwd_multi(int N, int C, int W, int H, const float* splats, const int32_t* vals_sorted,
+                                       const int32_t* tile_offsets, float* colors, float* alphas, int32_t* last_ids,
+                                       unsigned char* hit_mask, cudaStream_t stream) {
+    ADB_REQUIRE(N >= 0 && C > 0 && C <= 65535 && W > 0 && H > 0, "adb_raster_blend_fwd_multi: bad sizes");
+    ADB_REQUIRE(tile_offsets && colors && alphas && last_ids, "adb_raster_blend_fwd_multi: null pointer");
+    ADB_REQUIRE(N == 0 || splats, "adb_raster_blend_fwd_multi: null pointer");
+    return blend_fwd_impl(false, C, W, H, 0, splats, vals_sorted, tile_offsets, colors, alphas, last_ids, nullptr, hit_mask,
+                          stream);
 }
 
 // Legacy (Inria) blending: colors[...,3] = sum alpha*T/z (inverse depth); main_ids [H,W] may be NULL.
 ADB_API int adb_raster_blend_fwd_legacy(int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
                                         const int32_t* tile_offsets, float* colors, float* alphas, int32_t* last_ids,
                                         int32_t* main_ids, cudaStream_t stream) {
-    return blend_fwd_impl(true, W, H, n_per_cam, splats, vals_sorted, tile_offsets, colors, alphas, last_ids, main_ids,
-                          nullptr, stream);
+    return blend_fwd_single(true, W, H, n_per_cam, splats, vals_sorted, tile_offsets, colors, alphas, last_ids, main_ids,
+                            nullptr, stream);
 }
 
 template <bool LEGACY, int S, int OCC, bool ASYNC>
-static int launch_bwd(dim3 grid, int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
+static int launch_bwd(dim3 grid, int W, int H, int wrap, const float* splats, const int32_t* vals_sorted,
                       const int32_t* tile_offsets, const float* alphas, const int32_t* last_ids, const float* v_colors,
                       const float* v_alphas, float* v_splats, const unsigned char* hit_mask, cudaStream_t stream) {
     static AdbDeviceOnce once;
@@ -651,25 +684,22 @@ static int launch_bwd(dim3 grid, int W, int H, int n_per_cam, const float* splat
     });
     if (rc != ADB_OK) return rc;
     blend_bwd_kernel<LEGACY, S, OCC, ASYNC><<<grid, BLOCK, BwdSmem<S, ASYNC>::BYTES, stream>>>(
-        W, H, splats, vals_sorted, tile_offsets, n_per_cam, alphas, last_ids, v_colors, v_alphas, v_splats, hit_mask);
+        W, H, splats, vals_sorted, tile_offsets, wrap, alphas, last_ids, v_colors, v_alphas, v_splats, hit_mask);
     return ADB_OK;
 }
 
-static int blend_bwd_impl(bool legacy, int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
+// C views (gridDim.z); wrap: see record_index.
+static int blend_bwd_impl(bool legacy, int C, int W, int H, int wrap, const float* splats, const int32_t* vals_sorted,
                           const int32_t* tile_offsets, const float* alphas, const int32_t* last_ids,
                           const float* v_colors, const float* v_alphas, float* v_splats, const unsigned char* hit_mask,
                           cudaStream_t stream) {
-    ADB_REQUIRE(W > 0 && H > 0 && n_per_cam >= 0, "adb_raster_blend_bwd: bad sizes");
-    ADB_REQUIRE(tile_offsets && alphas && last_ids && v_colors && v_alphas, "adb_raster_blend_bwd: null pointer");
-    if (n_per_cam == 0) return ADB_OK;
-    ADB_REQUIRE(v_splats, "adb_raster_blend_bwd: null v_splats");
-    dim3 grid(adb_cdiv(W, ADB_TILE), adb_cdiv(H, ADB_TILE));
+    dim3 grid(adb_cdiv(W, ADB_TILE), adb_cdiv(H, ADB_TILE), C);
     // A/B switches: ADB_BWD_SLOTS=32 -> 32-slot deferred-reduction buffer (2 CTAs/SM);
     // ADB_BWD_OCC=3 -> 79 registers, 3 CTAs/SM instead of the default 64 registers, 4 CTAs/SM.
     static const int slots = getenv("ADB_BWD_SLOTS") ? atoi(getenv("ADB_BWD_SLOTS")) : 16;
     static const int occ = getenv("ADB_BWD_OCC") ? atoi(getenv("ADB_BWD_OCC")) : 4;
     int rc;
-#define ADB_BWD_ARGS grid, W, H, n_per_cam, splats, vals_sorted, tile_offsets, alphas, last_ids, v_colors, v_alphas, v_splats, hit_mask, stream
+#define ADB_BWD_ARGS grid, W, H, wrap, splats, vals_sorted, tile_offsets, alphas, last_ids, v_colors, v_alphas, v_splats, hit_mask, stream
     // ADB_BLEND_TMA=1: double-buffered cp.async.bulk staging (+13 KB of shared memory: 3 CTAs/SM instead of 4); opt-in for
     // the same reason as the forward kernel.
     static const int tma = getenv("ADB_BLEND_TMA") ? atoi(getenv("ADB_BLEND_TMA")) : 0;
@@ -684,13 +714,25 @@ static int blend_bwd_impl(bool legacy, int W, int H, int n_per_cam, const float*
     return ADB_OK;
 }
 
+static int blend_bwd_single(bool legacy, int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
+                            const int32_t* tile_offsets, const float* alphas, const int32_t* last_ids,
+                            const float* v_colors, const float* v_alphas, float* v_splats, const unsigned char* hit_mask,
+                            cudaStream_t stream) {
+    ADB_REQUIRE(W > 0 && H > 0 && n_per_cam >= 0, "adb_raster_blend_bwd: bad sizes");
+    ADB_REQUIRE(tile_offsets && alphas && last_ids && v_colors && v_alphas, "adb_raster_blend_bwd: null pointer");
+    if (n_per_cam == 0) return ADB_OK;
+    ADB_REQUIRE(v_splats, "adb_raster_blend_bwd: null v_splats");
+    return blend_bwd_impl(legacy, 1, W, H, n_per_cam, splats, vals_sorted, tile_offsets, alphas, last_ids, v_colors, v_alphas,
+                          v_splats, hit_mask, stream);
+}
+
 // v_splats [N,12] must be zeroed by the caller; gradients are accumulated into it.
 ADB_API int adb_raster_blend_bwd(int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
                                  const int32_t* tile_offsets, const float* alphas, const int32_t* last_ids,
                                  const float* v_colors, const float* v_alphas, float* v_splats,
                                  cudaStream_t stream) {
-    return blend_bwd_impl(false, W, H, n_per_cam, splats, vals_sorted, tile_offsets, alphas, last_ids, v_colors,
-                          v_alphas, v_splats, nullptr, stream);
+    return blend_bwd_single(false, W, H, n_per_cam, splats, vals_sorted, tile_offsets, alphas, last_ids, v_colors,
+                            v_alphas, v_splats, nullptr, stream);
 }
 
 // Same with the forward's culling decisions (adb_raster_blend_fwd_hits of the SAME splats / vals_sorted / tile_offsets): the
@@ -700,8 +742,23 @@ ADB_API int adb_raster_blend_bwd_hits(int W, int H, int n_per_cam, const float* 
                                       const float* v_colors, const float* v_alphas, float* v_splats,
                                       const unsigned char* hit_mask, cudaStream_t stream) {
     ADB_REQUIRE(hit_mask, "adb_raster_blend_bwd_hits: null hit_mask");
-    return blend_bwd_impl(false, W, H, n_per_cam, splats, vals_sorted, tile_offsets, alphas, last_ids, v_colors,
-                          v_alphas, v_splats, hit_mask, stream);
+    return blend_bwd_single(false, W, H, n_per_cam, splats, vals_sorted, tile_offsets, alphas, last_ids, v_colors,
+                            v_alphas, v_splats, hit_mask, stream);
+}
+
+// C views in one launch: buffers as adb_raster_blend_fwd_multi, v_colors [C,H,W,4], v_alphas [C,H,W], v_splats [C,N,12]
+// (zeroed by the caller, accumulated), hit_mask from adb_raster_blend_fwd_multi (may be NULL: the kernel then culls itself).
+// N = 0: nothing to accumulate, accepted without a launch.
+ADB_API int adb_raster_blend_bwd_multi(int N, int C, int W, int H, const float* splats, const int32_t* vals_sorted,
+                                       const int32_t* tile_offsets, const float* alphas, const int32_t* last_ids,
+                                       const float* v_colors, const float* v_alphas, float* v_splats,
+                                       const unsigned char* hit_mask, cudaStream_t stream) {
+    ADB_REQUIRE(N >= 0 && C > 0 && C <= 65535 && W > 0 && H > 0, "adb_raster_blend_bwd_multi: bad sizes");
+    ADB_REQUIRE(tile_offsets && alphas && last_ids && v_colors && v_alphas, "adb_raster_blend_bwd_multi: null pointer");
+    if (N == 0) return ADB_OK;
+    ADB_REQUIRE(splats && v_splats, "adb_raster_blend_bwd_multi: null pointer");
+    return blend_bwd_impl(false, C, W, H, 0, splats, vals_sorted, tile_offsets, alphas, last_ids, v_colors, v_alphas,
+                          v_splats, hit_mask, stream);
 }
 
 // Legacy (Inria) conventions; v_colors[...,3] is the upstream gradient of the inverse-depth channel and v_splats slot 9
@@ -710,6 +767,6 @@ ADB_API int adb_raster_blend_bwd_legacy(int W, int H, int n_per_cam, const float
                                         const int32_t* tile_offsets, const float* alphas, const int32_t* last_ids,
                                         const float* v_colors, const float* v_alphas, float* v_splats,
                                         cudaStream_t stream) {
-    return blend_bwd_impl(true, W, H, n_per_cam, splats, vals_sorted, tile_offsets, alphas, last_ids, v_colors,
-                          v_alphas, v_splats, nullptr, stream);
+    return blend_bwd_single(true, W, H, n_per_cam, splats, vals_sorted, tile_offsets, alphas, last_ids, v_colors,
+                            v_alphas, v_splats, nullptr, stream);
 }

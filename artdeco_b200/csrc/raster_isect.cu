@@ -11,6 +11,7 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cub/iterator/transform_input_iterator.cuh>
+#include <stdio.h>
 
 namespace {
 
@@ -175,6 +176,11 @@ ADB_API int adb_raster_tile_offsets(long long n_isect, const int64_t* keys_sorte
 // COPIES = 4 replicas of every tile counter (selected by CTA index) cut the same-address serialisation of the L2 atomics
 // that a single counter per tile suffers.
 //
+// Views: the scan, scatter and sort take C views at once (one scan CTA per view, a view grid dimension for the scatter,
+// (T, C) CTAs for the sort).  View c has its own counter block [2*COPIES*T] and tile_offsets row [T+1], and owns the segment
+// [base_c, base_c + cap_c) of the one packed/keys/vals buffer, base_c = sum of the previous views' capacities.  Offsets and
+// vals are absolute in that buffer, so the blend kernels index it directly; vals follow gsplat's cam*N + gaussian.
+//
 // Why the order equals the reference's stable radix sort of (tile, depth): the reference emits keys Gaussian-major, so
 // inside one (tile, depth) tie the stable sort leaves ascending Gaussian ids — exactly the ascending order of the
 // composite word (depth_bits, gaussian).  A Gaussian touches a tile at most once, so the words of a tile are distinct
@@ -184,6 +190,13 @@ namespace {
 
 constexpr int COPIES = ADB_TILE_COUNTER_COPIES;
 static_assert(COPIES == 4, "the scan kernel reads one tile's counters as an int4");
+constexpr int MAX_VIEWS = 64;
+
+// Per-view segments of the intersection buffer, passed by value (kernel parameters, so a captured graph keeps them).
+struct Segments {
+    long long base[MAX_VIEWS];
+    long long cap[MAX_VIEWS];
+};
 
 __global__ void __launch_bounds__(256)
 tile_count_kernel(int N, const int32_t* __restrict__ radii, const float* __restrict__ splats,
@@ -202,19 +215,25 @@ tile_count_kernel(int N, const int32_t* __restrict__ radii, const float* __restr
         for (int tx = x0; tx < x1; ++tx) atomicAdd(tile_counts + (ty * tw + tx) * COPIES + cp, 1);
 }
 
-// Single CTA, 1024 threads, over the T*COPIES counters in (tile-major, copy-minor) order.
-// starts[e] = min(capacity, sum_{f<e} counts[f]);  offsets[t] = starts[t*COPIES];  offsets[T] = min(capacity, total).
+// One CTA of 1024 threads per view, over the view's T*COPIES counters in (tile-major, copy-minor) order.
+// starts[e] = base + min(capacity, sum_{f<e} counts[f]);  offsets[t] = starts[t*COPIES];  offsets[T] = base + min(capacity, total).
+// offsets_all == NULL: only the totals are computed (nothing else written).
 // Each thread owns 16 consecutive counters (4 tiles x 4 copies): four 128-bit loads in flight, one block-wide scan of the
 // per-thread sums per 16384 counters (1080p: two rounds; the first version looped 8 times with
 // four barriers each and took 20 us).
 constexpr int SCAN_THREADS = 1024;
 __global__ void __launch_bounds__(SCAN_THREADS)
-tile_scan_kernel(int T, const int32_t* __restrict__ counts, long long capacity, int32_t* __restrict__ starts,
-                 int32_t* __restrict__ offsets, long long* __restrict__ total, int32_t* __restrict__ overflow) {
+tile_scan_kernel(int T, int32_t* __restrict__ counts_all, Segments seg, int32_t* __restrict__ offsets_all,
+                 long long* __restrict__ total, int32_t* __restrict__ overflow) {
     constexpr int PER = 16;                                  // 1024 threads x 16 counters = 16384 per round, no spills
     __shared__ long long s_warp[32];
     __shared__ long long s_carry;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int view = blockIdx.x;
+    const int32_t* counts = counts_all + (size_t)view * 2 * COPIES * T;
+    int32_t* starts = counts_all + (size_t)view * 2 * COPIES * T + (size_t)T * COPIES;
+    int32_t* offsets = offsets_all ? offsets_all + (size_t)view * (T + 1) : nullptr;
+    const long long capacity = seg.cap[view], seg_base = seg.base[view];
     const int E = T * COPIES;
     if (tid == 0) s_carry = 0;
     __syncthreads();
@@ -255,11 +274,11 @@ tile_scan_kernel(int T, const int32_t* __restrict__ counts, long long capacity, 
         for (int v = 0; v < PER / 4; ++v) {
             const int e = e0 + 4 * v;
             int4 st;
-            st.x = (int32_t)(excl < capacity ? excl : capacity); excl += c[4 * v];
-            st.y = (int32_t)(excl < capacity ? excl : capacity); excl += c[4 * v + 1];
-            st.z = (int32_t)(excl < capacity ? excl : capacity); excl += c[4 * v + 2];
-            st.w = (int32_t)(excl < capacity ? excl : capacity); excl += c[4 * v + 3];
-            if (e < E) {
+            st.x = (int32_t)(seg_base + (excl < capacity ? excl : capacity)); excl += c[4 * v];
+            st.y = (int32_t)(seg_base + (excl < capacity ? excl : capacity)); excl += c[4 * v + 1];
+            st.z = (int32_t)(seg_base + (excl < capacity ? excl : capacity)); excl += c[4 * v + 2];
+            st.w = (int32_t)(seg_base + (excl < capacity ? excl : capacity)); excl += c[4 * v + 3];
+            if (offsets && e < E) {
                 *reinterpret_cast<int4*>(starts + e) = st;
                 offsets[e / COPIES] = st.x;
             }
@@ -270,24 +289,29 @@ tile_scan_kernel(int T, const int32_t* __restrict__ counts, long long capacity, 
     }
     if (tid == 0) {
         const long long tot = s_carry;
-        offsets[T] = (int32_t)(tot < capacity ? tot : capacity);
-        if (total) *total = tot;
-        if (overflow && tot > capacity) *overflow = 1;
+        if (offsets) offsets[T] = (int32_t)(seg_base + (tot < capacity ? tot : capacity));
+        if (total) total[view] = tot;
+        if (overflow && offsets && tot > capacity) overflow[view] = 1;
     }
 }
 
 __global__ void __launch_bounds__(256)
 tile_scatter_kernel(int N, const int32_t* __restrict__ radii, const float* __restrict__ splats,
                     const int32_t* __restrict__ tiles_per_gauss, int W, int H, int convention,
-                    const int32_t* __restrict__ starts, int32_t* __restrict__ tile_counts, long long capacity,
-                    unsigned long long* __restrict__ packed) {
+                    int32_t* __restrict__ counts_all, Segments seg, unsigned long long* __restrict__ packed) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N) return;
-    if (tiles_per_gauss[i] <= 0) return;
-    const int2 r = reinterpret_cast<const int2*>(radii)[i];
-    const float2 m = reinterpret_cast<const float2*>(splats + (size_t)i * ADB_SPLAT_STRIDE)[0];
-    const float depth = splats[(size_t)i * ADB_SPLAT_STRIDE + 11];
+    const int view = blockIdx.y;
+    const size_t vi = (size_t)view * N + i;
+    if (tiles_per_gauss[vi] <= 0) return;
+    const int2 r = reinterpret_cast<const int2*>(radii)[vi];
+    const float2 m = reinterpret_cast<const float2*>(splats + vi * ADB_SPLAT_STRIDE)[0];
+    const float depth = splats[vi * ADB_SPLAT_STRIDE + 11];
     const int tw = (W + ADB_TILE - 1) / ADB_TILE;
+    const int T = tw * ((H + ADB_TILE - 1) / ADB_TILE);
+    int32_t* tile_counts = counts_all + (size_t)view * 2 * COPIES * T;
+    const int32_t* starts = tile_counts + (size_t)T * COPIES;
+    const long long seg_end = seg.base[view] + seg.cap[view];
     const int cp = blockIdx.x & (COPIES - 1);
     int x0, x1, y0, y1;
     adb_tile_rect(m.x, m.y, r.x, r.y, W, H, convention, x0, x1, y0, y1);
@@ -308,7 +332,7 @@ tile_scatter_kernel(int N, const int32_t* __restrict__ radii, const float* __res
         for (int u = 0; u < 4; ++u)
             if (e[u] >= 0) {
                 const long long slot = (long long)starts[e[u]] + (a[u] - 1);
-                if (slot < capacity) packed[slot] = word;
+                if (slot < seg_end) packed[slot] = word;
             }
     }
 }
@@ -443,10 +467,12 @@ __device__ __forceinline__ void bitonic_sort_global(volatile u64* a, int n, int 
 }
 
 __global__ void __launch_bounds__(SORT_THREADS)
-tile_sort_kernel(int T, const int32_t* __restrict__ offsets, u64* __restrict__ packed, int cam_id,
+tile_sort_kernel(int T, const int32_t* __restrict__ offsets_all, u64* __restrict__ packed, int cam0,
                  int n_per_cam, int tile_bits, int64_t* __restrict__ keys, int32_t* __restrict__ vals) {
     __shared__ u64 s_words[SORT_SMEM_CAP];
     const int tile = blockIdx.x;
+    const int cam_id = cam0 + blockIdx.y;
+    const int32_t* offsets = offsets_all + (size_t)blockIdx.y * (T + 1);
     const int start = offsets[tile], n = offsets[tile + 1] - start;
     if (n <= 0) return;
     const int tid = threadIdx.x;
@@ -461,7 +487,7 @@ tile_sort_kernel(int T, const int32_t* __restrict__ offsets, u64* __restrict__ p
         if (n > 1) bitonic_sort_shared(s_words, np2, tid);
         for (int i = tid; i < n; i += SORT_THREADS) {
             const u64 w = s_words[i];
-            keys[start + i] = (int64_t)(hi | (w >> 32));
+            if (keys) keys[start + i] = (int64_t)(hi | (w >> 32));
             vals[start + i] = vbase + (int32_t)(unsigned)(w & 0xffffffffu);
         }
     } else {
@@ -471,13 +497,60 @@ tile_sort_kernel(int T, const int32_t* __restrict__ offsets, u64* __restrict__ p
         __threadfence_block();
         for (int i = tid; i < n; i += SORT_THREADS) {
             const u64 w = g[i];
-            keys[start + i] = (int64_t)(hi | (w >> 32));
+            if (keys) keys[start + i] = (int64_t)(hi | (w >> 32));
             vals[start + i] = vbase + (int32_t)(unsigned)(w & 0xffffffffu);
         }
     }
 }
 
 }  // namespace
+
+// Fills the per-view segments from the host array of capacities; refuses what the int32 offsets cannot address.
+static int make_segments(const char* name, int C, const long long* capacities, Segments& seg) {
+    char msg[160];
+    if (!(C > 0 && C <= MAX_VIEWS)) {
+        snprintf(msg, sizeof(msg), "%s: C must be 1..%d", name, MAX_VIEWS);
+        adb_set_error_msg(msg);
+        return ADB_ERR_INVALID;
+    }
+    if (!capacities) {
+        snprintf(msg, sizeof(msg), "%s: null capacities", name);
+        adb_set_error_msg(msg);
+        return ADB_ERR_INVALID;
+    }
+    long long base = 0;
+    for (int c = 0; c < C; ++c) {
+        if (capacities[c] < 0 || base + capacities[c] >= 2147483647LL) {
+            snprintf(msg, sizeof(msg), "%s: capacities must be >= 0 and sum to less than 2^31 - 1", name);
+            adb_set_error_msg(msg);
+            return ADB_ERR_INVALID;
+        }
+        seg.base[c] = base;
+        seg.cap[c] = capacities[c];
+        base += capacities[c];
+    }
+    return ADB_OK;
+}
+
+static int scan_launch(int C, int T, int32_t* tile_counts, const Segments& seg, int32_t* tile_offsets, long long* total,
+                       int32_t* overflow, cudaStream_t stream) {
+    tile_scan_kernel<<<C, SCAN_THREADS, 0, stream>>>(T, tile_counts, seg, tile_offsets, total, overflow);
+    ADB_CHECK_LAUNCH("tile_scan_kernel");
+    return ADB_OK;
+}
+
+static int scatter_sort_launch(int N, int C, const int32_t* radii, const float* splats, const int32_t* tiles_per_gauss,
+                               int W, int H, int convention, int cam0, const Segments& seg, int32_t* tile_counts,
+                               const int32_t* tile_offsets, void* packed, int64_t* keys, int32_t* vals, cudaStream_t stream) {
+    const int T = adb_cdiv(W, ADB_TILE) * adb_cdiv(H, ADB_TILE);
+    tile_scatter_kernel<<<dim3(adb_cdiv(N, 256), C), 256, 0, stream>>>(N, radii, splats, tiles_per_gauss, W, H, convention,
+                                                                      tile_counts, seg, (unsigned long long*)packed);
+    ADB_CHECK_LAUNCH("tile_scatter_kernel");
+    tile_sort_kernel<<<dim3(T, C), SORT_THREADS, 0, stream>>>(T, tile_offsets, (unsigned long long*)packed, cam0, N,
+                                                             adb_tile_bits(W, H), keys, vals);
+    ADB_CHECK_LAUNCH("tile_sort_kernel");
+    return ADB_OK;
+}
 
 // tile_counts: int32 [2 * ADB_TILE_COUNTER_COPIES * T]: first half = the per-(tile,copy) counters, which must be all-zero
 // on entry (they are zero again after adb_raster_tile_scatter_sort: allocate + zero once); second half = segment starts
@@ -496,10 +569,10 @@ static int tile_bucket_impl(int convention, int N, const int32_t* radii, const f
                                                                tile_counts);
         ADB_CHECK_LAUNCH("tile_count_kernel");
     }
-    tile_scan_kernel<<<1, SCAN_THREADS, 0, stream>>>(T, tile_counts, capacity, tile_counts + (size_t)T * COPIES, tile_offsets, total,
-                                            overflow);
-    ADB_CHECK_LAUNCH("tile_scan_kernel");
-    return ADB_OK;
+    Segments seg;
+    seg.base[0] = 0;
+    seg.cap[0] = capacity;
+    return scan_launch(1, T, tile_counts, seg, tile_offsets, total, overflow, stream);
 }
 
 ADB_API int adb_raster_tile_count_scan(int N, const int32_t* radii, const float* splats, const int32_t* tiles_per_gauss,
@@ -516,6 +589,21 @@ ADB_API int adb_raster_tile_scan(int W, int H, long long capacity, int32_t* tile
                             overflow, 1, stream);
 }
 
+// C views in one launch (counters filled by adb_raster_project_fwd_multi).  capacities: HOST array [C]; view c's segment
+// of the intersection buffer starts at the sum of the previous capacities.  tile_counts [C, 2*4*T], tile_offsets [C, T+1]
+// (absolute indices into the buffer), total int64 [C] and overflow int32 [C] on the device (may be NULL).  tile_offsets ==
+// NULL computes the totals only (sizing pass: read them, then scan again with capacities = totals).
+ADB_API int adb_raster_tile_scan_multi(int C, int W, int H, const long long* capacities, int32_t* tile_counts,
+                                       int32_t* tile_offsets, long long* total, int32_t* overflow, cudaStream_t stream) {
+    Segments seg;
+    const int rc = make_segments("adb_raster_tile_scan_multi", C, capacities, seg);
+    if (rc != ADB_OK) return rc;
+    ADB_REQUIRE(W > 0 && H > 0, "adb_raster_tile_scan_multi: bad sizes");
+    ADB_REQUIRE(tile_counts && (tile_offsets || total), "adb_raster_tile_scan_multi: null pointer");
+    const int T = adb_cdiv(W, ADB_TILE) * adb_cdiv(H, ADB_TILE);
+    return scan_launch(C, T, tile_counts, seg, tile_offsets, total, overflow, stream);
+}
+
 // Scatter + per-tile sort.  keys [capacity] int64, vals [capacity] int32, packed [capacity] uint64 scratch; tile_counts as
 // left by adb_raster_tile_count_scan.
 ADB_API int adb_raster_tile_scatter_sort(int N, const int32_t* radii, const float* splats, const int32_t* tiles_per_gauss,
@@ -527,14 +615,28 @@ ADB_API int adb_raster_tile_scatter_sort(int N, const int32_t* radii, const floa
     if (N == 0 || capacity == 0) return ADB_OK;
     ADB_REQUIRE(radii && splats && tiles_per_gauss && tile_counts && tile_offsets && packed && keys && vals,
                 "adb_raster_tile_scatter_sort: null pointer");
-    const int T = adb_cdiv(W, ADB_TILE) * adb_cdiv(H, ADB_TILE);
-    tile_scatter_kernel<<<adb_cdiv(N, 256), 256, 0, stream>>>(N, radii, splats, tiles_per_gauss, W, H,
-                                                             legacy ? ADB_CONV_INRIA : ADB_CONV_GSPLAT,
-                                                             tile_counts + (size_t)T * COPIES, tile_counts, capacity,
-                                                             (unsigned long long*)packed);
-    ADB_CHECK_LAUNCH("tile_scatter_kernel");
-    tile_sort_kernel<<<T, SORT_THREADS, 0, stream>>>(T, tile_offsets, (unsigned long long*)packed, cam_id, N,
-                                                    adb_tile_bits(W, H), keys, vals);
-    ADB_CHECK_LAUNCH("tile_sort_kernel");
-    return ADB_OK;
+    ADB_REQUIRE(capacity < 2147483647LL, "adb_raster_tile_scatter_sort: bad sizes");
+    Segments seg;
+    seg.base[0] = 0;
+    seg.cap[0] = capacity;
+    return scatter_sort_launch(N, 1, radii, splats, tiles_per_gauss, W, H, legacy ? ADB_CONV_INRIA : ADB_CONV_GSPLAT, cam_id,
+                               seg, tile_counts, tile_offsets, packed, keys, vals, stream);
+}
+
+// C views in one scatter and one sort launch: radii [C,N,2], splats [C,N,12], tiles_per_gauss [C,N]; tile_counts and
+// tile_offsets as left by adb_raster_tile_scan_multi with the SAME host capacities [C].  packed / vals (and keys unless
+// NULL) hold sum(capacities) elements; view c's entries start at the sum of the previous capacities, vals = c*N + gaussian.
+ADB_API int adb_raster_tile_scatter_sort_multi(int N, int C, const int32_t* radii, const float* splats,
+                                               const int32_t* tiles_per_gauss, int W, int H, const long long* capacities,
+                                               int32_t* tile_counts, const int32_t* tile_offsets, void* packed,
+                                               int64_t* keys, int32_t* vals, cudaStream_t stream) {
+    Segments seg;
+    const int rc = make_segments("adb_raster_tile_scatter_sort_multi", C, capacities, seg);
+    if (rc != ADB_OK) return rc;
+    ADB_REQUIRE(N >= 0 && W > 0 && H > 0 && (long long)C * N < 2147483647LL, "adb_raster_tile_scatter_sort_multi: bad sizes");
+    if (N == 0) return ADB_OK;
+    ADB_REQUIRE(radii && splats && tiles_per_gauss && tile_counts && tile_offsets && packed && vals,
+                "adb_raster_tile_scatter_sort_multi: null pointer");
+    return scatter_sort_launch(N, C, radii, splats, tiles_per_gauss, W, H, ADB_CONV_GSPLAT, 0, seg, tile_counts, tile_offsets,
+                               packed, keys, vals, stream);
 }

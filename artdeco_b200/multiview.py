@@ -6,8 +6,9 @@ exchange, leaving on every rank the sum over ALL views of the per-view gradients
 losses"; the reference optimises one view per step, Reconstruct/scene/scene_models/h3dgsv3.py:406-464).
 
 Design:
-  * the whole local compute (projection -> tile-bucketed intersection -> blend fwd -> blend bwd, per view) has no host
-    sync (intersection buffers are sized by a capacity measured once) and is captured in ONE CUDA graph;
+  * the whole local compute (projection -> tile-bucketed intersection -> blend fwd -> blend bwd) runs stage by stage over
+    the batch, one launch per stage for all local views (raster.project_multi / intersect_multi / blend_*_multi); it has no
+    host sync (intersection buffers are sized by a capacity measured once) and is captured in ONE CUDA graph;
   * gradients are produced by the multi-view backward kernels (parameters read once, gradients written once);
   * multi-GPU: 12 B colour gradients all-gathered, 11 geometry floats all-reduced, both overlapped with the backward
     kernels, instead of a dense [N,59] all-reduce — by ``parallel.MultiViewExchange`` (NCCL, default) or ``peer.PeerExchange``
@@ -27,7 +28,7 @@ KEYS = ("means", "quats", "scales", "opacities", "sh")
 class MultiViewStep:
     def __init__(self, params: dict, viewmats: torch.Tensor, Ks: torch.Tensor, W: int, H: int, world: int = 1,
                  sh_degree: int = 3, eps2d: float = 0.01, near: float = 0.01, far: float = 1e10, radius_clip: float = 0.0,
-                 graph: bool = True, capacity_margin: float = 1.25, overlap_views: bool = False,
+                 graph: bool = True, capacity_margin: float = 1.25, overlap_views: bool = False,  # no effect
                  exchange_kind: str | None = None):
         """``params``: dict of the five parameter tensors on the device; ``viewmats [C,4,4]``, ``Ks [C,3,3]``: the LOCAL
         views (``parallel.views_for_rank``).  ``world`` > 1 needs an initialised process group; ``exchange_kind``: "nccl"
@@ -60,38 +61,58 @@ class MultiViewStep:
             self.grads.update(v_means=torch.empty(N, 3, device=dev), v_quats=torch.empty(N, 4, device=dev),
                               v_scales=torch.empty(N, 3, device=dev), v_opac=torch.empty(N, device=dev))
         self.grads["g_rgb"] = torch.empty(C, N, 3, dtype=torch.float32, device=dev)
+        T = ((W + R.TILE - 1) // R.TILE) * ((H + R.TILE - 1) // R.TILE)
+        self.counts = torch.zeros(C, 2 * R.COUNTER_COPIES * T, dtype=torch.int32, device=dev)   # per-view tile counters
+        self.n_dev = torch.zeros(C, dtype=torch.int64, device=dev)          # per-view intersection count ...
+        self.overflow_dev = torch.zeros(C, dtype=torch.int32, device=dev)   # ... and overflow flag of the last step
         self.capacity = None
         self.margin = capacity_margin
         self.use_graph = graph
-        # overlap_views=True runs consecutive views on two CUDA streams (the latency-bound projection / atomics / sort stages of
-        # one view could fill the gaps of the other's issue-bound blend kernels; both streams fork from / join the caller's, so
-        # the pair is capturable in one graph).  Off by default: co-running issue-bound blend kernels of two views compete for
-        # the same issue slots.
-        self.overlap_views = overlap_views and self.C > 1
-        self._side = torch.cuda.Stream(device=dev) if self.overlap_views else None
+        # No effect, kept because callers set it: every stage is one launch for the whole batch, so there are no per-view
+        # launches left to overlap on a second stream.
+        self.overlap_views = overlap_views
         self.graph = None
-        self.render = None          # (colors [C,H,W,4], alphas [C,H,W]) of the last step
-        self.info = None            # per view: {"n_isect": int64[1], "overflow": int32[1]} device tensors
+        self.render = None          # (colors [C,H,W,4], alphas [C,H,W]) of the last step (world > 1: per-view lists)
+        self.info = None            # {"n_isect": int64[C], "overflow": int32[C]} device tensors of the last step
         self.v_views = self.v_campos = None
 
     # ---- stages -----------------------------------------------------------------------------------------------------
-    def _view(self, c, capacity):
-        """projection -> intersection -> blend fwd -> blend bwd -> masked colour gradient of local view c."""
+    def _project(self):
+        """Projection + SH + tile counting of every local view in one pass over the parameters."""
         sh_degree, eps2d, near, far, rclip = self.cfg
-        p, W, H, N = self.p, self.W, self.H, self.N
-        self.v_splats[c].zero_()
-        cnt = R.new_tile_counts(W, H, self.dev)        # per-tile counting is fused into the projection kernel
-        R.project(p["means"], p["quats"], p["scales"], p["opacities"], p["sh"], sh_degree, self.V[c], self.K[c], self.P[c],
-                  W, H, eps2d, near, far, rclip, out=(self.radii[c], self.splats[c], self.tpg[c]), tile_counts=cnt)
-        cap = None if capacity is None else capacity[c]
-        keys, vals, offs, info = R.intersect(self.radii[c], self.splats[c], self.tpg[c], W, H, capacity=cap, counts=cnt)
+        p = self.p
+        self.counts.zero_()
+        R.project_multi(p["means"], p["quats"], p["scales"], p["opacities"], p["sh"], sh_degree, self.V, self.K, self.P,
+                        self.W, self.H, eps2d, near, far, rclip, self.counts, out=(self.radii, self.splats, self.tpg))
+
+    def _raster(self, views, capacity):
+        """intersection -> blend fwd -> blend bwd of the local views ``views`` (a slice), one launch per stage."""
+        W, H = self.W, self.H
+        caps = None if capacity is None else capacity[views]
+        self.v_splats[views].zero_()
+        _, vals, offs, _, seg = R.intersect_multi(self.radii[views], self.splats[views], self.tpg[views], W, H,
+                                                  self.counts[views], capacities=caps, keys=False,
+                                                  info={"n_isect": self.n_dev[views], "overflow": self.overflow_dev[views]})
         hits = R.new_hit_mask(vals)                    # the forward's culling decisions, reused by the backward
-        col, alp, last = R.blend_forward(W, H, N, self.splats[c], vals, offs, hits=hits)
-        R.blend_backward(W, H, N, self.splats[c], vals, offs, alp, last, self.v_colors[c], self.v_alphas[c],
-                         out=self.v_splats[c], hits=hits)
-        if self.exchange is not None and not self._fused_push:
+        col, alp, last = R.blend_forward_multi(W, H, self.splats[views], vals, offs, hits=hits)
+        R.blend_backward_multi(W, H, self.splats[views], vals, offs, alp, last, self.v_colors[views], self.v_alphas[views],
+                               out=self.v_splats[views], hits=hits)
+        return col, alp, seg
+
+    def _local_views(self, capacity):
+        """Every local view as one batch; no host sync when capacity is given."""
+        self._project()
+        return self._raster(slice(0, self.C), capacity)
+
+    def _view(self, c, capacity):
+        """Multi-GPU route: intersection -> blend fwd -> blend bwd -> masked colour gradient of local view c alone, so that its
+        gather can start as soon as its blend backward has finished.  The projection of all views runs before view 0."""
+        if c == 0:
+            self._project()
+        col, alp, _ = self._raster(slice(c, c + 1), capacity)
+        if not self._fused_push:
             R.mask_rgb_grad(self.splats[c], self.v_splats[c], self.grads["g_rgb"][c])
-        return col, alp, info, (keys, vals, offs, last)
+        return col[0], alp[0]
 
     def _gather_view(self, c):
         """Hands local view c's colour gradient to the exchange as soon as its blend backward has been issued."""
@@ -101,25 +122,6 @@ class MultiViewStep:
         else:
             self.exchange.start_gather_view(c, self.grads["g_rgb"][c], campos)
 
-    def _local_views(self, capacity):
-        """Every local view; no host sync when capacity is given."""
-        cols, alps, infos = [None] * self.C, [None] * self.C, [None] * self.C
-        cur = torch.cuda.current_stream(self.dev)
-        two = self.overlap_views and capacity is not None       # the calibration pass syncs per view: keep it on one stream
-        if two:
-            self._side.wait_stream(cur)
-        for c in range(self.C):
-            st = self._side if (two and (c & 1)) else cur
-            with torch.cuda.stream(st):
-                col, alp, info, tmp = self._view(c, capacity)
-                if two and st is not cur:
-                    for tns in tmp + (col, alp):
-                        tns.record_stream(cur)
-            cols[c], alps[c], infos[c] = col, alp, info
-        if two:
-            cur.wait_stream(self._side)
-        return cols, alps, infos
-
     def _backward(self):
         p = self.p
         out = R.multi_view_backward(p["means"], p["quats"], p["scales"], p["sh"], self.cfg[0], self.V, self.K, self.P, self.W,
@@ -127,11 +129,10 @@ class MultiViewStep:
         self.v_views, self.v_campos = out[5], out[6]
 
     def calibrate(self):
-        """One eager pass with host syncs: measures the intersection count of every local view and fixes the capacities."""
+        """One eager pass with one host sync: measures the intersection count of every local view and fixes the capacities."""
         with torch.cuda.device(self.dev):
-            _, _, infos = self._local_views(None)
+            _, _, counts = self._local_views(None)
             self._backward()
-        counts = [int(i) for i in infos]
         self.capacity = [int(n * self.margin) + 4096 for n in counts]
         self.n_isect = counts
         return counts
@@ -141,32 +142,35 @@ class MultiViewStep:
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):                     # warm-up off the capture stream
-            self._local_views(self.capacity)
             if self.exchange is None:
+                self._local_views(self.capacity)
                 self._backward()
+            else:
+                for c in range(self.C):
+                    self._view(c, self.capacity)
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
+        self.info = {"n_isect": self.n_dev, "overflow": self.overflow_dev}
         if self.exchange is None:
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                cols, alps, infos = self._local_views(self.capacity)
+                col, alp, _ = self._local_views(self.capacity)
                 self._backward()
-            self.graph, self.render, self.info = [g], (cols, alps), infos
+            self.graph, self.render = [g], (col, alp)
             return
         # multi-GPU: one graph PER VIEW, so that view c's colour gradients can be all-gathered (NCCL, outside the graphs)
-        # while view c+1 renders
-        graphs, cols, alps, infos = [], [], [], []
+        # while view c+1 renders; graph 0 also holds the projection of every local view
+        graphs, cols, alps = [], [], []
         pool = None
         for c in range(self.C):
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g, pool=pool):
-                col, alp, info, _ = self._view(c, self.capacity)
+                col, alp = self._view(c, self.capacity)
             pool = g.pool()
             graphs.append(g)
             cols.append(col)
             alps.append(alp)
-            infos.append(info)
-        self.graph, self.render, self.info = graphs, (cols, alps), infos
+        self.graph, self.render = graphs, (cols, alps)
 
     # ---- public -----------------------------------------------------------------------------------------------------
     def set_upstream(self, v_colors: torch.Tensor, v_alphas: torch.Tensor):
@@ -190,16 +194,18 @@ class MultiViewStep:
                         g.replay()
                         self._gather_view(c)
                     self._backward()                    # 2 kernels + the all-reduce, eager (NCCL outside the graphs)
+            elif self.exchange is None:
+                col, alp, _ = self._local_views(self.capacity)
+                self.render, self.info = (col, alp), {"n_isect": self.n_dev, "overflow": self.overflow_dev}
+                self._backward()
             else:
-                cols, alps, infos = [], [], []
+                cols, alps = [], []
                 for c in range(self.C):
-                    col, alp, info, _ = self._view(c, self.capacity)
-                    if self.exchange is not None:
-                        self._gather_view(c)
+                    col, alp = self._view(c, self.capacity)
+                    self._gather_view(c)
                     cols.append(col)
                     alps.append(alp)
-                    infos.append(info)
-                self.render, self.info = (cols, alps), infos
+                self.render, self.info = (cols, alps), {"n_isect": self.n_dev, "overflow": self.overflow_dev}
                 self._backward()
         return self.grads
 
@@ -207,8 +213,8 @@ class MultiViewStep:
         """Host sync.  Raises if any view's intersection count exceeded its capacity since the last check."""
         if self.info is None:
             return self.n_isect
-        counts = [int(i["n_isect"]) for i in self.info]
-        if any(int(i["overflow"]) for i in self.info):
+        counts = [int(n) for n in self.info["n_isect"].tolist()]
+        if int(self.info["overflow"].max()):
             raise _lib.ArtdecoB200Error(f"intersection capacity exceeded: counts {counts}, capacities {self.capacity}; "
                                         "call calibrate() again (the scene grew)")
         self.n_isect = counts

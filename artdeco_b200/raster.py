@@ -49,6 +49,14 @@ _lib.register("adb_raster_blend_bwd_hits", [i32, i32, i32, vp, vp, vp, vp, vp, v
 _lib.register("adb_raster_blend_fwd_legacy", [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp])
 _lib.register("adb_raster_blend_bwd_legacy", [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp])
 
+_caps_t = C.POINTER(C.c_longlong)
+_lib.register("adb_raster_project_fwd_multi", [i32, i32, vp, vp, vp, vp, vp, i32, vp, vp, vp, i32, i32, f32, f32, f32, f32,
+                                               vp, vp, vp, vp, vp])
+_lib.register("adb_raster_tile_scan_multi", [i32, i32, i32, _caps_t, vp, vp, vp, vp, vp])
+_lib.register("adb_raster_tile_scatter_sort_multi", [i32, i32, vp, vp, vp, i32, i32, _caps_t, vp, vp, vp, vp, vp, vp])
+_lib.register("adb_raster_blend_fwd_multi", [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp])
+_lib.register("adb_raster_blend_bwd_multi", [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp])
+
 
 TILE = 16
 SPLAT_STRIDE = 12
@@ -103,10 +111,108 @@ def project(means, quats, scales, opacities, sh, sh_degree, viewmat, K, campos, 
     return radii, splats, tpg
 
 
-def new_tile_counts(W, H, dev):
-    """Zeroed counter buffer of the tile-bucketed intersection: 4 replicated counters per tile, then their segment starts."""
+def new_tile_counts(W, H, dev, views=None):
+    """Zeroed counter buffer of the tile-bucketed intersection: 4 replicated counters per tile, then their segment starts.
+    ``views``: C -> one such block per view, [C, 2*4*T] (``project_multi`` / ``intersect_multi``)."""
     T = ((W + TILE - 1) // TILE) * ((H + TILE - 1) // TILE)
-    return torch.zeros(2 * COUNTER_COPIES * T, dtype=torch.int32, device=dev)
+    shape = (2 * COUNTER_COPIES * T,) if views is None else (int(views), 2 * COUNTER_COPIES * T)
+    return torch.zeros(shape, dtype=torch.int32, device=dev)
+
+
+# ---- the multi-view batch, stage by stage: one launch per stage for C views of the same Gaussians ----------------------------
+def project_multi(means, quats, scales, opacities, sh, sh_degree, viewmats, Ks, camposs, W, H, eps2d, near, far, radius_clip,
+                  tile_counts, out=None):
+    """Projection + SH + fused tile counting of C cameras in one pass (parameters read once).  ``viewmats [C,4,4]``,
+    ``Ks [C,3,3]``, ``camposs [C,3]``; ``tile_counts`` from ``new_tile_counts(..., views=C)``.  Returns radii [C,N,2],
+    splats [C,N,12], tiles_per_gauss [C,N], per view bit-identical to ``project(..., tile_counts=...)``."""
+    N, Cn, dev = means.shape[0], viewmats.shape[0], means.device
+    if out is not None:
+        radii, splats, tpg = out
+    else:
+        radii = torch.empty(Cn, N, 2, dtype=torch.int32, device=dev)
+        splats = torch.empty(Cn, N, SPLAT_STRIDE, dtype=torch.float32, device=dev)
+        tpg = torch.empty(Cn, N, dtype=torch.int32, device=dev)
+    _lib.call("adb_raster_project_fwd_multi", N, Cn, _lib.ptr(means), _lib.ptr(quats), _lib.ptr(scales), _lib.ptr(opacities),
+              _lib.ptr(sh), int(sh_degree), _lib.ptr(viewmats), _lib.ptr(Ks), _lib.ptr(camposs), W, H, eps2d, near, far,
+              radius_clip, _lib.ptr(radii), _lib.ptr(splats), _lib.ptr(tpg), _lib.ptr(tile_counts), _lib.stream())
+    return radii, splats, tpg
+
+
+def intersect_multi(radii, splats, tpg, W, H, counts, capacities=None, keys=True, info=None):
+    """Tile-bucketed intersection of C views (``radii [C,N,2]`` ...; ``counts`` filled by ``project_multi``): one scan, one
+    scatter and one sort launch.  View c owns the segment ``[sum(seg[:c]), +seg[c])`` of one keys / vals buffer; offsets
+    [C,T+1] are absolute indices into it and vals = c*N + gaussian (gsplat's concatenated per-camera layout).
+
+    ``capacities=None``: one host sync reads all C counts and the segments are exactly the counts.  ``capacities`` (C ints):
+    no host sync; entries of a view beyond its count are undefined, and a view that needed more is flagged in
+    ``info["overflow"][c]`` (its image is then incomplete; the other views are unaffected).
+    ``keys=False``: the sort writes vals only (keys is then None).  ``info``: optional preallocated
+    ``{"n_isect": int64[C], "overflow": int32[C]}``.  Returns ``(keys, vals, offsets, info, seg)``; ``seg`` = the segment
+    sizes (all zero when N = 0)."""
+    Cn, N = radii.shape[0], radii.shape[1]
+    dev = radii.device
+    T = ((W + TILE - 1) // TILE) * ((H + TILE - 1) // TILE)
+    if info is None:
+        info = {"n_isect": torch.zeros(Cn, dtype=torch.int64, device=dev),
+                "overflow": torch.zeros(Cn, dtype=torch.int32, device=dev)}
+    else:
+        info["n_isect"].zero_()
+        info["overflow"].zero_()
+    offsets = torch.empty(Cn, T + 1, dtype=torch.int32, device=dev)
+    if capacities is None:
+        zero = (C.c_longlong * Cn)(*([0] * Cn))
+        _lib.call("adb_raster_tile_scan_multi", Cn, W, H, zero, _lib.ptr(counts), None, _lib.ptr(info["n_isect"]), None,
+                  _lib.stream())
+        seg = [int(n) for n in info["n_isect"].tolist()]        # the pipeline's single host sync
+        if sum(seg) >= 2147483647:
+            raise _lib.ArtdecoB200Error("more than 2^31 tile intersections in the batch")
+    else:
+        seg = [int(c) for c in capacities]
+        if len(seg) != Cn:
+            raise ValueError(f"intersect_multi: {len(seg)} capacities for {Cn} views")
+        if N == 0:
+            seg = [0] * Cn                       # no Gaussians, no intersections: nothing to pad
+    caps = (C.c_longlong * Cn)(*seg)
+    _lib.call("adb_raster_tile_scan_multi", Cn, W, H, caps, _lib.ptr(counts), _lib.ptr(offsets), _lib.ptr(info["n_isect"]),
+              _lib.ptr(info["overflow"]), _lib.stream())
+    total = sum(seg)
+    vals = torch.empty(max(total, 1), dtype=torch.int32, device=dev)
+    keys_t = torch.empty(max(total, 1), dtype=torch.int64, device=dev) if keys else None
+    packed = torch.empty(max(total, 1), dtype=torch.int64, device=dev)
+    _lib.call("adb_raster_tile_scatter_sort_multi", N, Cn, _lib.ptr(radii), _lib.ptr(splats), _lib.ptr(tpg), W, H, caps,
+              _lib.ptr(counts), _lib.ptr(offsets), _lib.ptr(packed), _lib.ptr(keys_t), _lib.ptr(vals), _lib.stream())
+    return (keys_t[:total] if keys else None), vals[:total], offsets, info, seg
+
+
+def blend_forward_multi(W, H, splats, vals, offsets, hits=None, out=None):
+    """Blend forward of C views in one launch (``splats [C,N,12]``, ``vals`` / ``offsets`` from ``intersect_multi``).
+    Returns colors [C,H,W,4], alphas [C,H,W], last_ids [C,H,W] (absolute sorted indices).  ``hits``: ``new_hit_mask(vals)``."""
+    Cn, dev = splats.shape[0], splats.device
+    if out is not None:
+        colors, alphas, last_ids = out
+    else:
+        colors = torch.empty(Cn, H, W, 4, dtype=torch.float32, device=dev)
+        alphas = torch.empty(Cn, H, W, dtype=torch.float32, device=dev)
+        last_ids = torch.empty(Cn, H, W, dtype=torch.int32, device=dev)
+    if hits is not None and (hits.dtype != torch.uint8 or hits.numel() < vals.numel() or hits.device != dev):
+        raise ValueError("blend_forward_multi: hits must be a uint8 tensor with one byte per intersection (new_hit_mask)")
+    _lib.call("adb_raster_blend_fwd_multi", splats.shape[1], Cn, W, H, _lib.ptr(splats),
+              _lib.ptr(vals) if vals.numel() else None,
+              _lib.ptr(offsets), _lib.ptr(colors), _lib.ptr(alphas), _lib.ptr(last_ids), _lib.ptr(hits), _lib.stream())
+    return colors, alphas, last_ids
+
+
+def blend_backward_multi(W, H, splats, vals, offsets, alphas, last_ids, v_colors, v_alphas, out=None, hits=None):
+    """Blend backward of C views in one launch.  ``out``: optional ZEROED [C,N,12] accumulator; ``hits``: the mask
+    ``blend_forward_multi`` filled for the same buffers."""
+    v_splats = out if out is not None else torch.zeros_like(splats)
+    if hits is not None and (hits.dtype != torch.uint8 or hits.numel() < vals.numel() or hits.device != splats.device):
+        raise ValueError("blend_backward_multi: hits must be the uint8 mask blend_forward_multi filled for these intersections")
+    _lib.call("adb_raster_blend_bwd_multi", splats.shape[1], splats.shape[0], W, H, _lib.ptr(splats),
+              _lib.ptr(vals) if vals.numel() else None,
+              _lib.ptr(offsets), _lib.ptr(alphas), _lib.ptr(last_ids), _lib.ptr(v_colors), _lib.ptr(v_alphas),
+              _lib.ptr(v_splats), _lib.ptr(hits), _lib.stream())
+    return v_splats
 
 
 def intersect(radii, splats, tpg, W, H, cam_id=0, n_cams=1, sort=True, legacy=False, capacity=None, method=None, counts=None):
@@ -303,71 +409,52 @@ class _RasterizeOneCamera(torch.autograd.Function):
 
 
 class _RasterizeCameras(torch.autograd.Function):
-    """C > 1 cameras of the same Gaussians (BASELINE config 4: an 8-view batch per optimiser step).  Forward: the
-    single-view stages per camera into stacked buffers.  Backward: blend_bwd per camera, then ONE multi-view projection
-    backward (parameters read once, 11 geometry gradients summed in registers) and ONE multi-view SH backward (v_sh
-    written once) instead of C single-view passes plus C-1 [N,59] accumulations (csrc/raster_project_bwd_multi.cu)."""
+    """C > 1 cameras of the same Gaussians (BASELINE config 4: an 8-view batch per optimiser step), stage by stage: one
+    multi-view projection (parameters read once), one view-batched intersection, one blend forward launch for all views.
+    Backward: one blend backward launch, then ONE multi-view projection backward (11 geometry gradients summed in registers)
+    and ONE multi-view SH backward (v_sh written once) (csrc/raster_project_bwd_multi.cu)."""
 
     @staticmethod
     def forward(ctx, means, quats, scales, opacities, sh, viewmats, Ks, camposs, W, H, sh_degree, eps2d, near, far,
                 radius_clip, exchange=None, capacities=None):
         _lib.require_cuda(means)
         ctx.exchange = exchange
-        N, Cn = means.shape[0], viewmats.shape[0]
+        Cn = viewmats.shape[0]
         dev = means.device
         with torch.cuda.device(dev):
-            radii = torch.empty(Cn, N, 2, dtype=torch.int32, device=dev)
-            splats = torch.empty(Cn, N, SPLAT_STRIDE, dtype=torch.float32, device=dev)
-            tpg = torch.empty(Cn, N, dtype=torch.int32, device=dev)
-            colors = torch.empty(Cn, H, W, 4, dtype=torch.float32, device=dev)
-            alphas = torch.empty(Cn, H, W, dtype=torch.float32, device=dev)
-            last_ids = torch.empty(Cn, H, W, dtype=torch.int32, device=dev)
-            keys_l, vals_l, offs_l, infos, hits_l = [], [], [], [], []
-            for c in range(Cn):
-                cnt = new_tile_counts(W, H, dev) if N > 0 else None
-                project(means, quats, scales, opacities, sh, sh_degree, viewmats[c], Ks[c], camposs[c], W, H, eps2d, near,
-                        far, radius_clip, out=(radii[c], splats[c], tpg[c]), tile_counts=cnt)
-                cap = None if capacities is None else int(capacities[c] if hasattr(capacities, "__len__") else capacities)
-                keys, vals, offsets, info = intersect(radii[c], splats[c], tpg[c], W, H, c, Cn, capacity=cap, counts=cnt)
-                hits = new_hit_mask(vals)
-                blend_forward(W, H, N, splats[c], vals, offsets, out=(colors[c], alphas[c], last_ids[c]), hits=hits)
-                hits_l.append(hits)
-                keys_l.append(keys)
-                vals_l.append(vals)
-                offs_l.append(offsets)
-                infos.append(info)
+            cnt = new_tile_counts(W, H, dev, Cn)
+            radii, splats, tpg = project_multi(means, quats, scales, opacities, sh, sh_degree, viewmats, Ks, camposs, W, H,
+                                               eps2d, near, far, radius_clip, cnt)
+            caps = None
+            if capacities is not None:
+                caps = [int(c) for c in capacities] if hasattr(capacities, "__len__") else [int(capacities)] * Cn
+            keys, vals, offsets, info, _ = intersect_multi(radii, splats, tpg, W, H, cnt, capacities=caps)
+            hits = new_hit_mask(vals)
+            colors, alphas, last_ids = blend_forward_multi(W, H, splats, vals, offsets, hits=hits)
         ctx.save_for_backward(means, quats, scales, opacities, sh, viewmats, Ks, camposs, radii, splats, alphas, last_ids,
-                              *vals_l, *offs_l)
-        ctx.cfg = (W, H, sh_degree, Cn)
-        ctx.hits = hits_l
-        isect_ids, flatten_ids = torch.cat(keys_l), torch.cat(vals_l)
-        base, offs_out = 0, []
-        for c in range(Cn):                        # gsplat offsets index the concatenated list (padded in capacity mode)
-            offs_out.append(offs_l[c][:-1] + base)
-            base += int(vals_l[c].numel())
-        isect_offsets = torch.stack(offs_out)
+                              vals, offsets)
+        ctx.cfg = (W, H, sh_degree)
+        ctx.hits = hits
+        # gsplat offsets index the concatenated list (padded per camera in capacity mode): the segment layout of intersect_multi
+        isect_offsets = offsets[:, :-1].contiguous()
         if capacities is None:
             overflow = torch.zeros(1, dtype=torch.int32, device=dev)
         else:
-            overflow = torch.stack([i["overflow"] for i in infos]).amax(0)
-        ctx.mark_non_differentiable(radii, splats, tpg, isect_ids, flatten_ids, isect_offsets, overflow)
-        return colors, alphas, radii, splats, tpg, isect_ids, flatten_ids, isect_offsets, overflow
+            overflow = info["overflow"].amax().reshape(1)
+        ctx.mark_non_differentiable(radii, splats, tpg, keys, vals, isect_offsets, overflow)
+        return colors, alphas, radii, splats, tpg, keys, vals, isect_offsets, overflow
 
     @staticmethod
     def backward(ctx, v_colors, v_alphas, *_unused):
-        W, H, sh_degree, Cn = ctx.cfg
-        saved = ctx.saved_tensors
-        means, quats, scales, opacities, sh, viewmats, Ks, camposs, radii, splats, alphas, last_ids = saved[:12]
-        vals_l, offs_l = saved[12:12 + Cn], saved[12 + Cn:12 + 2 * Cn]
-        N = means.shape[0]
+        W, H, sh_degree = ctx.cfg
+        (means, quats, scales, opacities, sh, viewmats, Ks, camposs, radii, splats, alphas, last_ids, vals,
+         offsets) = ctx.saved_tensors
+        Cn = viewmats.shape[0]
         dev = means.device
         v_colors = torch.zeros(Cn, H, W, 4, device=dev) if v_colors is None else _f32c(v_colors)
         v_alphas = torch.zeros(Cn, H, W, device=dev) if v_alphas is None else _f32c(v_alphas)
         with torch.cuda.device(dev):
-            v_splats = torch.zeros(Cn, N, SPLAT_STRIDE, dtype=torch.float32, device=dev)
-            for c in range(Cn):
-                blend_backward(W, H, N, splats[c], vals_l[c], offs_l[c], alphas[c], last_ids[c], v_colors[c], v_alphas[c],
-                               out=v_splats[c], hits=ctx.hits[c])
+            v_splats = blend_backward_multi(W, H, splats, vals, offsets, alphas, last_ids, v_colors, v_alphas, hits=ctx.hits)
             ex = ctx.exchange
             grads = multi_view_backward(means, quats, scales, sh, sh_degree, viewmats, Ks, camposs, W, H, radii, splats,
                                         v_splats, out=(dict(ex.views) if ex is not None else None), exchange=ex)

@@ -54,6 +54,14 @@ int adb_raster_project_fwd_counts(int N, const float* means, const float* quats,
                                   const float* K, const float* campos, int W, int H, float eps2d, float near_plane,
                                   float far_plane, float radius_clip, int32_t* radii, float* splats,
                                   int32_t* tiles_per_gauss, int32_t* tile_counts, adb_stream_t stream);
+/* C views of the same Gaussians in one pass: viewmats [C,16], Ks [C,9], camposs [C,3] (device); radii [C,N,2], splats [C,N,12],
+ * tiles_per_gauss [C,N], tile_counts [C,2*4*T] (first half of every block zero on entry).  Per view bit-identical to
+ * adb_raster_project_fwd_counts; the parameters (and the SH coefficients) are read once. */
+int adb_raster_project_fwd_multi(int N, int C, const float* means, const float* quats, const float* scales,
+                                 const float* opacities, const float* sh, int sh_degree, const float* viewmats,
+                                 const float* Ks, const float* camposs, int W, int H, float eps2d, float near_plane,
+                                 float far_plane, float radius_clip, int32_t* radii, float* splats,
+                                 int32_t* tiles_per_gauss, int32_t* tile_counts, adb_stream_t stream);
 int adb_raster_scan_workspace_bytes(int N, size_t* bytes /*HOST*/);
 int adb_raster_isect_scan(int N, const int32_t* tiles_per_gauss, int64_t* cum_tiles /*[N] inclusive*/, void* ws,
                           size_t ws_bytes, adb_stream_t stream);
@@ -107,6 +115,19 @@ int adb_raster_tile_scan(int W, int H, long long capacity, int32_t* tile_counts,
 int adb_raster_tile_scatter_sort(int N, const int32_t* radii, const float* splats, const int32_t* tiles_per_gauss, int W, int H,
                                  int legacy, int cam_id, int n_cams, long long capacity, int32_t* tile_counts,
                                  const int32_t* tile_offsets, void* packed, int64_t* keys, int32_t* vals, adb_stream_t stream);
+/* View-batched intersection (one launch per stage for C views; 1 <= C <= 64).  capacities: HOST array [C]; view c owns the
+ * segment [sum_{c'<c} capacities[c'], +capacities[c]) of one packed / keys / vals buffer (the sum must stay below 2^31 - 1).
+ *   adb_raster_tile_scan_multi         one CTA per view: tile_offsets [C,T+1] ABSOLUTE in that buffer, clamped to the view's
+ *                                      capacity; total int64 [C] and overflow int32 [C] (SET when total[c] > capacities[c])
+ *                                      on the device.  tile_offsets == NULL: totals only (a sizing pass).
+ *   adb_raster_tile_scatter_sort_multi scatter (view grid dimension) + per-tile sort over (T, C) CTAs; vals = c*N + gaussian;
+ *                                      keys (may be NULL: not written) = c|tile|depth_bits as adb_raster_tile_scatter_sort. */
+int adb_raster_tile_scan_multi(int C, int W, int H, const long long* capacities /*HOST [C]*/, int32_t* tile_counts,
+                               int32_t* tile_offsets, long long* total, int32_t* overflow, adb_stream_t stream);
+int adb_raster_tile_scatter_sort_multi(int N, int C, const int32_t* radii, const float* splats, const int32_t* tiles_per_gauss,
+                                       int W, int H, const long long* capacities /*HOST [C]*/, int32_t* tile_counts,
+                                       const int32_t* tile_offsets, void* packed, int64_t* keys, int32_t* vals,
+                                       adb_stream_t stream);
 int adb_raster_blend_fwd(int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
                          const int32_t* tile_offsets, float* colors /*[H,W,4]*/, float* alphas /*[H,W]*/,
                          int32_t* last_ids /*[H,W]*/, adb_stream_t stream);
@@ -124,6 +145,17 @@ int adb_raster_blend_fwd_hits(int W, int H, int n_per_cam, const float* splats, 
 int adb_raster_blend_bwd_hits(int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
                               const int32_t* tile_offsets, const float* alphas, const int32_t* last_ids, const float* v_colors,
                               const float* v_alphas, float* v_splats, const unsigned char* hit_mask, adb_stream_t stream);
+/* View-batched blend pair (gridDim.z = C): splats [C,N,12] and v_splats [C,N,12] indexed by vals_sorted (c*N + gaussian)
+ * directly, tile_offsets [C,T+1] from adb_raster_tile_scan_multi, colors / v_colors [C,H,W,4], alphas / last_ids / v_alphas
+ * [C,H,W]; hit_mask (may be NULL) indexed like vals_sorted.  Per view the same images as the single-view _hits pair; last_ids
+ * are absolute sorted indices.  N = 0 (empty scene): the forward writes empty images (splats may be NULL), the backward
+ * returns without a launch. */
+int adb_raster_blend_fwd_multi(int N, int C, int W, int H, const float* splats, const int32_t* vals_sorted,
+                               const int32_t* tile_offsets, float* colors, float* alphas, int32_t* last_ids,
+                               unsigned char* hit_mask, adb_stream_t stream);
+int adb_raster_blend_bwd_multi(int N, int C, int W, int H, const float* splats, const int32_t* vals_sorted,
+                               const int32_t* tile_offsets, const float* alphas, const int32_t* last_ids, const float* v_colors,
+                               const float* v_alphas, float* v_splats, const unsigned char* hit_mask, adb_stream_t stream);
 int adb_raster_project_bwd(int N, const float* means, const float* quats, const float* scales, const float* sh,
                            int sh_degree, const float* viewmat, const float* K, const float* campos, int W, int H,
                            float eps2d, float near_plane, float far_plane, float radius_clip, const int32_t* radii,
