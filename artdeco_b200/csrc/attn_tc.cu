@@ -324,10 +324,11 @@ int make_map(CUtensorMap* map, const void* ptr, long long batch, int rows, int c
 }  // namespace
 
 // O[b, n, h*64 + d] = sum_k softmax_k(scale * <Q[b,h,n,:], K[b,h,k,:]>) * V[b,h,k,d]   (head_dim 64)
-//   Q: bf16 split [B*heads, Nq, 64];  K: [B*heads, Nk, 64];  Vt: [B*heads, 64, Nkpad] (Nkpad % 8 == 0, zero padded);
-//   O: bf16 split [B, Nq, heads*64].  *_lo all non-NULL selects bf16x3.
+//   Q: bf16 split [B*heads, Nq, 64];  K: [B*heads, Nk, 64];  Vt: [B*heads, 64, Nkpad] (Nkpad % 8 == 0; the padding
+//   columns need only be finite: keys >= Nk get weight exactly 0);  O: bf16 split [B, Nq, heads*64].
+//   Q/K/Vt *_lo all non-NULL selects bf16x3; O_lo is written whenever it is given.
 // 0 = automatic (default, currently variant 1; env ADB_ATTN_KERNEL overrides at load), 1 = one query tile per CTA, 2 = two query tiles per
-// persistent CTA.  Returns the previous setting.  Both variants produce the same values to rounding (tests/test_gemm.py).
+// persistent CTA.  Returns the previous setting.  Both variants produce bit-identical values (tests/test_tensorcore_edges.py).
 static std::atomic<int> g_attn_variant{getenv("ADB_ATTN_KERNEL") ? atoi(getenv("ADB_ATTN_KERNEL")) : 0};
 ADB_API int adb_attention_set_variant(int variant) {
     if (variant < 0 || variant > 2) return -1;
@@ -341,6 +342,8 @@ ADB_API int adb_attention_bf16(int B, int heads, int Nq, int Nk, int Nkpad, cons
     ADB_REQUIRE(Q_hi && K_hi && Vt_hi && O_hi, "adb_attention_bf16: null pointer");
     const bool x3 = Q_lo && K_lo && Vt_lo;
     ADB_REQUIRE(x3 || (!Q_lo && !K_lo && !Vt_lo), "adb_attention_bf16: give all lo operands or none");
+    ADB_REQUIRE((((uintptr_t)Q_hi | (uintptr_t)Q_lo | (uintptr_t)K_hi | (uintptr_t)K_lo | (uintptr_t)Vt_hi |
+                  (uintptr_t)Vt_lo) % 16) == 0, "adb_attention_bf16: operands must be 16-byte aligned");
     ADB_REQUIRE((((uintptr_t)O_hi | (uintptr_t)O_lo) % 16) == 0, "adb_attention_bf16: outputs must be 16-byte aligned");
     CUtensorMap mQh, mQl, mKh, mKl, mVh, mVl;
     const long long bh = (long long)B * heads;

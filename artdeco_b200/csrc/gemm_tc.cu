@@ -520,6 +520,8 @@ ADB_API int adb_conv3x3_bf16(int B, int H, int W, int Cin, int Cout, const void*
     ADB_REQUIRE(x_hi && w_hi && (D || D_hi), "adb_conv3x3_bf16: null pointer");
     ADB_REQUIRE((x_lo == nullptr) == (w_lo == nullptr), "adb_conv3x3_bf16: x_lo and w_lo must be given together");
     ADB_REQUIRE(act == 0 || act == 2, "adb_conv3x3_bf16: act must be 0 or 2 (ReLU)");
+    ADB_REQUIRE((((uintptr_t)x_hi | (uintptr_t)x_lo | (uintptr_t)w_hi | (uintptr_t)w_lo) % 16) == 0,
+                "adb_conv3x3_bf16: operands must be 16-byte aligned");
     GemmParams p{};
     p.nterms = x_lo ? 3 : 1;
     int wb = 128;

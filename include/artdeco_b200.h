@@ -23,7 +23,7 @@ typedef struct CUstream_st* adb_stream_t; /* == cudaStream_t */
 /* ---- library ---- */
 const char* adb_last_error(void);
 int adb_version(void);
-int adb_check_device(void); /* 0 iff the current device is compute capability 10.x */
+int adb_check_device(void); /* 0 iff the current device is compute capability 9.0 */
 
 /* ---- fused SSIM ----
  * replaces fused_ssim_cuda.fusedssim          Reconstruct/submodules/fused-ssim/ssim.cu:434-478 (ext.cpp:5)
@@ -316,13 +316,16 @@ int adb_gemm_bf16(int batch, int M, int N, int K, const void* A_hi, const void* 
                   long long sO2, long long sR2, adb_stream_t stream);
 /* adb_conv3x3_bf16: 3x3 / stride 1 / pad 1 convolution as an implicit GEMM on the same kernel (4-D TMA boxes, no im2col):
  *   replaces the nn.Conv2d(k=3) calls of croco/models/dpt_block.py:20-77,93-112,368-372.  x NHWC bf16 split, w bf16 split
- *   [Cout][9*Cin_pad] tap-major with Cin padded to 64; outputs NHWC; act 0/2 (ReLU); split_relu: split stores relu(v). */
+ *   [Cout][9*Cin_pad] tap-major with Cin padded to 64, x and w 16-byte aligned; outputs NHWC; act 0/2 (ReLU);
+ *   split_relu: split stores relu(v).  Any W >= 1 works: the pixel tile's TMA box may be wider than the image. */
 int adb_conv3x3_bf16(int B, int H, int W, int Cin, int Cout, const void* x_hi, const void* x_lo, const void* w_hi,
                      const void* w_lo, const float* bias, const float* residual, float* D, void* D_hi, void* D_lo, int act,
                      int split_relu, adb_stream_t stream);
 /* adb_attention_bf16: fused softmax(scale * Q K^T) V with the score matrix held in registers; replaces the three
  *   materialised torch ops at croco/models/blocks.py:105-109 (self) and :162-166 (cross).  head_dim 64.
- *   Q [B*heads,Nq,64], K [B*heads,Nk,64], Vt [B*heads,64,Nkpad] bf16 splits; O bf16 split [B,Nq,heads*64]. */
+ *   Q [B*heads,Nq,64], K [B*heads,Nk,64], Vt [B*heads,64,Nkpad] bf16 splits, 16-byte aligned; O bf16 split
+ *   [B,Nq,heads*64].  Keys >= Nk get weight exactly 0, so Vt's padding columns [Nk, Nkpad) need not be zero, only finite
+ *   (0 * Inf would still be NaN).  O_lo may be given in single pass (no Q/K/Vt lo parts) too. */
 int adb_attention_bf16(int B, int heads, int Nq, int Nk, int Nkpad, const void* Q_hi, const void* Q_lo, const void* K_hi,
                        const void* K_lo, const void* Vt_hi, const void* Vt_lo, float scale, void* O_hi, void* O_lo,
                        adb_stream_t stream);

@@ -27,10 +27,14 @@ def test_gemm_bf16x3_matches_fp64(cuda, M, N, K):
     ref2 = torch.nn.functional.gelu(0.5 * ref + bias.double()) + res.double()
     assert rel_err(out, ref2) < 2e-5
     assert rel_err(sp.hi.float() + sp.lo.float(), out) < 2e-5   # hi+lo keeps 16 mantissa bits
-    # single-pass bf16 (the fast mode) is only bf16-accurate
-    ops.gemm(ops.split(a, x3=False), ops.split(w, x3=False), M, N, K, out=out)
+    # single-pass bf16 (the fast mode) is only bf16-accurate ...
+    a1, w1 = ops.split(a, x3=False), ops.split(w, x3=False)
+    ops.gemm(a1, w1, M, N, K, out=out)
     e1 = rel_err(out, ref)
     assert 1e-4 < e1 < 2e-2
+    # ... but exact for its own bf16 operands up to fp32 accumulation, element by element (tests/test_tensorcore_edges.py)
+    ah, wh = a1.hi.double(), w1.hi.double()
+    assert ((out.double() - ah @ wh.T).abs() <= 3e-6 * (ah.abs() @ wh.abs().T)).all()
 
 
 @pytest.mark.gpu
