@@ -266,6 +266,59 @@ int adb_gauss_newton(int mode, int n_poses, int n_pts, int n_edges, float* poses
                      const unsigned char* valid_match, const float* Q, int height, int width, int pixel_border, float z_eps,
                      float sigma_a, float sigma_b, float C_thresh, float Q_thresh, int max_iter, float delta_thresh,
                      float* dx_out, int* state_out, void* ws, size_t ws_bytes, adb_stream_t stream);
+/* Frame tracking: CameraTracker.track after matching (VSLAM/CameraTracker.py:53-155), calibrated Sim(3) only
+ * (optimize_focal is not supported).  N = height * width points in KEY-FRAME pixel order; poses [8] = (t, q xyzw, s).
+ * Three calls on one stream share `ws` and the device `state` block; none synchronises the host:
+ *   adb_track_prepare  steps 2-5: Qk, the validity masks, constrain_points_to_ray, the 5x5 box-filter covariance and
+ *                      meas_k (get_points_poses, :189-219; utils_uncertainty.py:5-50), the match-fraction test (:83-118).
+ *   adb_track_solve    opt_pose_calib_sim3 (:296-396): Gauss-Newton with the covariance filter, convergence test
+ *                      (nonlinear_optimizer.py:5-25) and T_WCf = quat2unit(T_WCk T_CkCf) (:134).
+ *   adb_track_finish   step 6-7: point fusion into the key frame (:136-141, ImageFrame.py:30-48), check_keyframe and
+ *                      check_keyframe_map (:144-186). */
+enum { ADB_TRACK_OK = 0, ADB_TRACK_LOST_MATCHES = 1, ADB_TRACK_LOST_CHOLESKY = 2, ADB_TRACK_LOST_ZERO_COST = 3 };
+typedef struct adb_track_state {
+    int32_t lost;            /* ADB_TRACK_*: insufficient matches, non-positive pivot, zero previous cost */
+    int32_t iters;           /* Gauss-Newton iterations run */
+    int32_t converged;       /* check_convergence stopped the loop */
+    int32_t done;            /* the loop has stopped (converged or lost): remaining iterations are no-ops */
+    int32_t n_valid_opt, n_valid_kf, n_unique;   /* valid_opt.sum(), valid_kf.sum(), |unique(idx_f2k[valid_match_k])| */
+    int32_t is_keyframe, is_keyframe_map;
+    float tau_norm;          /* |tau| of the last iteration */
+    float cov_threshold;     /* max(quantile(det, 0.9), 1) of the last iteration (covariance filter) */
+    float dist_quantile;     /* quantile(|uv_f - uv_k| over valid_opt, thres_keyframe) */
+    double cost;             /* 0.5 b^T b of the last iteration (at the pose before its update) */
+    double prev_cost;        /* cost of the iteration before */
+    double last_dist;        /* last_dist after the key-frame tests */
+    double H[49], g[7];      /* normal equations of the last iteration: H = A^T A, g = -A^T b */
+    float T_CkCf[8];         /* current relative pose */
+    float T_WCk[8];          /* quat2unit(T_WCk) */
+} adb_track_state;
+/* ws_bytes (HOST) for N points; state_bytes (HOST) = sizeof(adb_track_state). */
+int adb_track_workspace_bytes(int n_pts, size_t* ws_bytes /*HOST*/, size_t* state_bytes /*HOST*/);
+/* idx_f2k int64 [N] (values in [0, N)), valid_match_k bool [N]; Xff [N,3], Cff [N], Qff [N] in frame order; Qkf [N];
+ * kf_X [N,3], kf_C [N], kf_N int32 [1] = the key frame's X_canon, C, N; K3x3 row-major.  Writes Xf, Xf_cov (the diagonal,
+ * [N,3]), Qk, meas_k [N,3], valid_meas_k / valid_opt / valid_kf (bool [N]) in key-frame order, and resets `state`
+ * (lost = ADB_TRACK_LOST_MATCHES when valid_opt.sum() / N < min_match_frac).  height, width >= 3 (reflect padding). */
+int adb_track_prepare(int height, int width, const float* K3x3, const long long* idx_f2k, const unsigned char* valid_match_k,
+                      const float* Xff, const float* Cff, const float* Qff, const float* Qkf, const float* kf_X,
+                      const float* kf_C, const int32_t* kf_N, float C_conf, float Q_conf, float depth_eps, float min_match_frac,
+                      float* Xf, float* Xf_cov, float* Qk, float* meas_k, unsigned char* valid_meas_k, unsigned char* valid_opt,
+                      unsigned char* valid_kf, adb_track_state* state, void* ws, size_t ws_bytes, adb_stream_t stream);
+/* Inputs as get_points_poses returns them (Xf_cov = diagonal [N,3]); T_WCf / T_WCk as stored (quat2unit is applied here).
+ * `state` must come from adb_track_prepare or be zeroed.  A fixed sequence of max_iters iterations, each a no-op once
+ * state->done is set.  On success T_WCf_out = quat2unit(T_WCk T_CkCf) and T_CkCf_out = the solution; on a lost outcome
+ * T_WCf_out is not written and T_CkCf_out holds the starting pose quat2unit(T_WCk)^-1 quat2unit(T_WCf). */
+int adb_track_solve(int n_pts, int height, int width, const float* K3x3, const float* Xf, const float* Xf_cov, const float* Qk,
+                    const unsigned char* valid, const float* meas_k, const unsigned char* valid_meas_k, const float* T_WCf,
+                    const float* T_WCk, int max_iters, int covariance_filter, int pixel_border, float depth_eps,
+                    float sigma_pixel, float sigma_depth, float huber_k, double rel_error, float delta_norm, float* T_WCf_out,
+                    float* T_CkCf_out, adb_track_state* state, void* ws, size_t ws_bytes, adb_stream_t stream);
+/* After adb_track_solve on the same state.  Unless lost: point fusion when point_fusion != 0 (kf_X, kf_C, kf_N updated in
+ * place with Xkf [N,3] and Ckf [N] through state->T_CkCf), then the key-frame tests; last_dist is the caller's value. */
+int adb_track_finish(int height, int width, const long long* idx_f2k, const unsigned char* valid_opt, const float* Xkf,
+                     const float* Ckf, float* kf_X, float* kf_C, int32_t* kf_N, int point_fusion, double match_frac_thresh,
+                     float thres_keyframe, double min_displacement, double last_dist, adb_track_state* state, void* ws,
+                     size_t ws_bytes, adb_stream_t stream);
 /* update_voxel (Reconstruct/scene/scene_models/h3dgsv3.py:227-316): voxel-hash class ids without the reference's three sorts
  * (csrc/voxel.cu).  Tables are caller-allocated: vkeys[V], pkeys[P], ukeys[U] uint64 pre-filled with 0xFF bytes; pcount[P]
  * int32 and best[V] uint64 zeroed; V, P powers of two >= 2N, U >= 2M.  mn = device float[3] minimum over all points.
