@@ -605,6 +605,9 @@ blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
 static int blend_fwd_impl(bool legacy, int C, int W, int H, int wrap, const float* splats, const int32_t* vals_sorted,
                           const int32_t* tile_offsets, float* colors, float* alphas, int32_t* last_ids,
                           int32_t* main_ids, unsigned char* hit_mask, cudaStream_t stream) {
+    // records are read as float4 (or by 48-byte bulk copies) and colours stored as float4: a misaligned view would fault
+    ADB_REQUIRE((((uintptr_t)splats | (uintptr_t)colors) % 16) == 0,
+                "adb_raster_blend_fwd: splats and colors must be 16-byte aligned");
     dim3 grid(adb_cdiv(W, ADB_TILE), adb_cdiv(H, ADB_TILE), C);
     // ADB_BLEND_TMA=1: double-buffered cp.async.bulk (TMA) staging.  Default: synchronous LDG staging (the kernel is
     // issue-bound with 4 CTAs/SM hiding the gather latency, so the extra prescale pass and mbarrier waits buy nothing).
@@ -693,6 +696,9 @@ static int blend_bwd_impl(bool legacy, int C, int W, int H, int wrap, const floa
                           const int32_t* tile_offsets, const float* alphas, const int32_t* last_ids,
                           const float* v_colors, const float* v_alphas, float* v_splats, const unsigned char* hit_mask,
                           cudaStream_t stream) {
+    // float4 record and upstream loads, red.global.add.v4 into the accumulators: a misaligned view would fault
+    ADB_REQUIRE((((uintptr_t)splats | (uintptr_t)v_colors | (uintptr_t)v_splats) % 16) == 0,
+                "adb_raster_blend_bwd: splats, v_colors and v_splats must be 16-byte aligned");
     dim3 grid(adb_cdiv(W, ADB_TILE), adb_cdiv(H, ADB_TILE), C);
     // A/B switches: ADB_BWD_SLOTS=32 -> 32-slot deferred-reduction buffer (2 CTAs/SM);
     // ADB_BWD_OCC=3 -> 79 registers, 3 CTAs/SM instead of the default 64 registers, 4 CTAs/SM.
