@@ -11,11 +11,12 @@ Public operators (same names / argument meaning as the reference's, see each mod
   optimizers.BaseAdam, optimizers.SparseGaussianAdam   (Reconstruct/scene/optimizers.py: fused step, one-launch add_and_prune)
   legacy.GaussianRasterizer, legacy.rasterize_gaussians  (diff_gaussian_rasterization legacy API, web viewer)
   tracking.track, tracking.opt_pose_calib_sim3         (VSLAM/CameraTracker.py: the Frontend's per-frame Sim(3) tracker)
+  densify.add_new_gaussians, densify.sample_lod        (SceneModel.add_new_gaussians: key-frame densification)
 There is no CPU implementation: every operator raises unless a CUDA sm_90 device and the C-ABI library
 ``libartdeco_b200.so`` are available.
 """
 from . import _lib  # noqa: F401
-from . import adam, covmlp, cull, gn, knn, legacy, mast3r, matching, multiview, optimizers, parallel, peer, raster, scene, tracking, voxel  # noqa: F401  (each registers its C signatures)
+from . import adam, covmlp, cull, densify, gn, knn, legacy, mast3r, matching, multiview, optimizers, parallel, peer, raster, scene, tracking, voxel  # noqa: F401  (each registers its C signatures)
 from .adam import adamUpdate, adamUpdateBasic  # noqa: F401
 from .covmlp import cov_mlp_modulate  # noqa: F401
 from .cull import lod_cull, lod_select, weed_out_mask  # noqa: F401

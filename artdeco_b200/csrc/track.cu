@@ -12,6 +12,7 @@
 //                     check_convergence.
 // Every sum has a fixed order and the histograms count integers, so results are bitwise reproducible run to run.
 #include "common.cuh"
+#include "select.cuh"
 #include "sim3.cuh"
 #include "artdeco_b200.h"
 
@@ -19,12 +20,16 @@ namespace {
 
 using adb_sim3::act_so3;
 using adb_sim3::quat_comp;
+using adb_select::HIST_BINS;
+using adb_select::SEL_THREADS;
+using adb_select::hist_add;
+using adb_select::hist_find;
+using adb_select::key_value;
+using adb_select::order_key;
 
 constexpr int TR_THREADS = 256;
 constexpr int TR_MAX_BLOCKS = 1024;       // reduce grid cap: fixed by N only, so the summation order is device-independent
 constexpr int TR_NSUM = 36;               // 28 (upper triangle of A^T A) + 7 (A^T b) + 1 (b^T b)
-constexpr int HIST_BINS = 65536;
-constexpr int SEL_THREADS = 1024;
 
 struct Sel {                               // selection state (workspace)
     unsigned int bin[2];                   // high 16 bits of the two order statistics
@@ -57,21 +62,6 @@ __device__ __forceinline__ void inv_sim3(const float* A, float* out) {
     act_so3(qi, A, t);
     out[0] = -si * t[0]; out[1] = -si * t[1]; out[2] = -si * t[2];
     out[3] = qi[0]; out[4] = qi[1]; out[5] = qi[2]; out[6] = qi[3]; out[7] = si;
-}
-
-// float -> uint32 whose unsigned order is the float order; every NaN maps to the largest key (torch.sort puts NaN last)
-__device__ __forceinline__ unsigned int order_key(float f) {
-    if (f != f) return 0xFFFFFFFFu;
-    const unsigned int b = __float_as_uint(f);
-    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-// hist[bin] += 1 with one atomic per distinct bin of the warp (neighbouring pixels mostly share a bin)
-__device__ __forceinline__ void hist_add(unsigned int* hist, unsigned int bin) {
-    const unsigned int peers = __match_any_sync(__activemask(), bin);
-    if ((threadIdx.x & 31) == (unsigned int)(__ffs(peers) - 1)) atomicAdd(hist + bin, (unsigned int)__popc(peers));
-}
-__device__ __forceinline__ float key_value(unsigned int k) {
-    return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k);
 }
 
 // ================================ preparation ================================
@@ -202,38 +192,6 @@ struct SelParams {
 };
 
 __device__ bool sel_active(int mode, const adb_track_state* st) { return mode == 0 ? st->done == 0 : st->lost == 0; }
-
-// rank r of a histogram -> (bin, rank inside the bin); one CTA of SEL_THREADS threads, each owning HIST_BINS/SEL_THREADS bins
-__device__ void hist_find(unsigned int* __restrict__ hist, const unsigned int* ranks, unsigned int* bins,
-                          unsigned int* in_bin, int n_ranks, unsigned int* s_tot) {
-    constexpr int PER = HIST_BINS / SEL_THREADS;
-    const int t = threadIdx.x;
-    unsigned int loc = 0;
-    for (int b = 0; b < PER; ++b) loc += hist[t * PER + b];
-    // inclusive scan of the per-thread totals (Hillis-Steele over shared memory)
-    s_tot[t] = loc;
-    __syncthreads();
-    for (int off = 1; off < SEL_THREADS; off <<= 1) {
-        const unsigned int v = t >= off ? s_tot[t - off] : 0u;
-        __syncthreads();
-        s_tot[t] += v;
-        __syncthreads();
-    }
-    const unsigned int excl = s_tot[t] - loc;
-    for (int k = 0; k < n_ranks; ++k) {
-        const unsigned int r = ranks[k];
-        if (r >= excl && r < excl + loc) {
-            unsigned int c = excl;
-            for (int b = 0; b < PER; ++b) {
-                const unsigned int h = hist[t * PER + b];
-                if (r < c + h) { bins[k] = t * PER + b; in_bin[k] = r - c; break; }
-                c += h;
-            }
-        }
-    }
-    __syncthreads();
-    for (int b = 0; b < PER; ++b) hist[t * PER + b] = 0u;
-}
 
 __device__ __forceinline__ void sel_ranks(const SelParams& p, const adb_track_state* st, int* n_out, unsigned int* r,
                                           float* w) {

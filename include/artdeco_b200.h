@@ -335,6 +335,33 @@ int adb_voxel_rank_new(long long M, int n, const void* sorted, const void* ukeys
                        const int* uslot_of, long long base, long long* cls_out, adb_stream_t stream);
 /* weed_out_gaussians (Reconstruct/scene/scene_models/h3dgsv3.py:942-953) for ALL key frames in one pass: cams [K,3] camera
  * centres (device); keep[i] = (#{k : |xyz_i - cam_k| < 2 d_max_i} / K > visible_threshold); visible_count [N] may be NULL. */
+/* Key-frame densification: the sampler of SceneModel.add_new_gaussians (Reconstruct/scene/scene_models/h3dgsv3.py:766-940,
+ * csrc/densify.cu).  One workspace (adb_densify_workspace_bytes for the LoD-1 image, height x width) serves every call.
+ *   adb_densify_depth_quantile  out[0] = torch.quantile(values[n], q) (linear, NaN if any value is NaN),
+ *                               out[1] = fp32(min(0.01, out[0])) as Python's min evaluates it (a NaN quantile gives 0.01)
+ *   adb_densify_sample          one LoD (1, 2, 4 or 8) of an image of height x width: init_proba [h,w] (get_lapla_norm of the
+ *                               resized image, x init_proba_scaler), penalty [h,w] (the same of the exposed render; may be NULL;
+ *                               0 without a render), flags [h,w] (bit 0 sampled, bit 1 valid) and *n_rows (device) = pixels
+ *                               with both bits.  image [3,H,W]; render [3,H,W] raw RGB with element strides render_strides[3]
+ *                               (HOST: channel, row, column) or NULL; exposure [3,4]; depth, conf [Hs,Ws]; uniforms [h,w];
+ *                               qmin [1] (out[1] above).  h = height / lod, w = width / lod, both >= 2.
+ *   adb_densify_emit            after adb_densify_sample on the same workspace: the *n_rows rows in row-major pixel order.
+ *                               cam [15] = R [3,3] row-major, t [3], approx_centre [3]; f the focal length in pixels.
+ *                               xyz [n,3], f_dc [n,3], scaling [n,3], opacity [n], d_max [n].
+ *   adb_densify_prune_mask      mask[i] = sigmoid(opacity[i]) > 0.05 && f max(exp(scaling[i])) / |xyz[i] - approx_centre| < 0.5 width */
+int adb_densify_workspace_bytes(int height, int width, size_t* bytes /*HOST*/);
+int adb_densify_depth_quantile(long long n, const float* values, float q, float* out /*[2]*/, void* ws, size_t ws_bytes,
+                               adb_stream_t stream);
+int adb_densify_sample(int height, int width, int lod, const float* image, const float* render,
+                       const long long* render_strides /*HOST [3]*/, const float* exposure, int Hs, int Ws, const float* depth,
+                       const float* conf, const float* uniforms, const float* qmin, float init_proba_scaler, float gs_add_ratio,
+                       float* init_proba, float* penalty, unsigned char* flags, int32_t* n_rows, void* ws, size_t ws_bytes,
+                       adb_stream_t stream);
+int adb_densify_emit(int height, int width, int lod, const float* image, int Hs, int Ws, const float* depth, const float* conf,
+                     const float* init_proba, const unsigned char* flags, const float* cam, double f, float* xyz, float* f_dc,
+                     float* scaling, float* opacity, float* d_max, void* ws, size_t ws_bytes, adb_stream_t stream);
+int adb_densify_prune_mask(long long N, const float* xyz, const float* opacity, const float* scaling,
+                           const float* approx_centre, double f, int width, unsigned char* mask, adb_stream_t stream);
 int adb_lod_weed_out(long long N, const float* xyz, const float* d_max, int K, const float* cams, float visible_threshold,
                      int32_t* visible_count, unsigned char* keep, adb_stream_t stream);
 
