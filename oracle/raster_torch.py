@@ -26,8 +26,18 @@ SH_C0 = 0.2820947917738781
 SH_C1 = 0.48860251190292
 
 
-def quat_to_rotmat(q: torch.Tensor) -> torch.Tensor:
-    q = q / q.norm(dim=-1, keepdim=True)
+MUTATIONS = ("fxfy_J", "lx_swap", "band_unclamped", "no_dotq", "no_qinv")
+
+
+def quat_to_rotmat(q: torch.Tensor, mutation: str | None = None) -> torch.Tensor:
+    n = q.norm(dim=-1, keepdim=True)
+    if mutation == "no_dotq":      # same value; gradient v/|q| instead of (v - <v,q^> q^)/|q|
+        q = (q / n).detach() + (q - q.detach()) / n.detach()
+    elif mutation == "no_qinv":    # same value; gradient (v - <v,q^> q^) without the 1/|q|
+        qn = q / n
+        q = qn.detach() + (qn - qn.detach()) * n.detach()
+    else:
+        q = q / n
     w, x, y, z = q.unbind(-1)
     return torch.stack([
         1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y),
@@ -35,25 +45,37 @@ def quat_to_rotmat(q: torch.Tensor) -> torch.Tensor:
         2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)], dim=-1).reshape(-1, 3, 3)
 
 
-def project(means, quats, scales, opacities, viewmat, K, W, H, eps2d=0.01, near=0.01, far=1e10, radius_clip=0.0):
-    """Returns radii[N,2] (int32), means2d[N,2], depths[N], conics[N,3] (differentiable where defined)."""
+def project(means, quats, scales, opacities, viewmat, K, W, H, eps2d=0.01, near=0.01, far=1e10, radius_clip=0.0,
+            mutation=None):
+    """Returns radii[N,2] (int32), means2d[N,2], depths[N], conics[N,3] (differentiable where defined).
+
+    ``mutation`` (one of MUTATIONS) plants a known bug, so that tests can show they would catch it: fx and fy swapped
+    in the Jacobian; the guard-band limits lxp and lxn swapped; the unclamped derivative of the Jacobian used in the
+    guard band; the quaternion normalisation backward without its ``- <v,q^> q^`` term or without its ``1/|q|``."""
+    assert mutation is None or mutation in MUTATIONS, mutation
     fx, fy, cx, cy = K[0, 0], K[1, 1], K[0, 2], K[1, 2]
     R, t = viewmat[:3, :3], viewmat[:3, 3]
     p = means @ R.T + t
     x, y, z = p.unbind(-1)
-    Rq = quat_to_rotmat(quats)
+    Rq = quat_to_rotmat(quats, mutation)
     M = Rq * scales[:, None, :]
     Sigma = M @ M.transpose(1, 2)
     Sc = R @ Sigma @ R.T
     tanx, tany = 0.5 * W / fx, 0.5 * H / fy
     lxp, lxn = (W - cx) / fx + 0.3 * tanx, cx / fx + 0.3 * tanx
     lyp, lyn = (H - cy) / fy + 0.3 * tany, cy / fy + 0.3 * tany
+    if mutation == "lx_swap":
+        lxp, lxn = lxn, lxp
     zs = torch.where(z.abs() > 1e-12, z, torch.full_like(z, 1e-12))
     rz = 1.0 / zs
     tx = zs * torch.minimum(lxp, torch.maximum(-lxn, x * rz))
     ty = zs * torch.minimum(lyp, torch.maximum(-lyn, y * rz))
+    if mutation == "band_unclamped":     # clamped value, derivative of the unclamped x and y
+        tx = tx.detach() + (x - x.detach())
+        ty = ty.detach() + (y - y.detach())
+    jx, jy = (fy, fx) if mutation == "fxfy_J" else (fx, fy)
     zero = torch.zeros_like(rz)
-    J = torch.stack([fx * rz, zero, -fx * tx * rz * rz, zero, fy * rz, -fy * ty * rz * rz], -1).reshape(-1, 2, 3)
+    J = torch.stack([jx * rz, zero, -jx * tx * rz * rz, zero, jy * rz, -jy * ty * rz * rz], -1).reshape(-1, 2, 3)
     S2 = J @ Sc @ J.transpose(1, 2)
     means2d = torch.stack([fx * x * rz + cx, fy * y * rz + cy], -1)
     a = S2[:, 0, 0] + eps2d
