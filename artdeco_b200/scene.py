@@ -11,7 +11,8 @@ What runs differently from the reference's ~30 torch kernels before the rasteriz
     when it is (training);
   * ``mlp_cov`` is the fused kernel of ``covmlp.cov_mlp_modulate`` (csrc/cov_mlp.cu).
 Same return dict as the reference: ``render [3,H,W]``, ``invdepth [1,H,W]``, ``visibility_filter [N0]``,
-``global_visibility_filter [n_cls]`` (when class ids are given), ``scale``.
+``global_visibility_filter [n_cls]`` (when class ids are given), ``scale``; plus the raw rasterizer outputs ``colors [1,H,W,4]``
+(RGB + accumulated depth) and ``alphas [1,H,W,1]``, which ``mapper.mapper_loss`` consumes (call with ``bg=None`` for that).
 """
 from __future__ import annotations
 
@@ -75,7 +76,8 @@ def render_lod(width: int, height: int, view_matrix: torch.Tensor, *, xyz, opaci
     visible_mask = torch.zeros(N0, dtype=torch.bool, device=dev)
     visible_mask[idx] = meta["radii"][0].max(dim=1).values > 0
     out = {"render": rendered_color[0], "invdepth": invdepth[0], "visibility_filter": visible_mask, "scale": sc_s,
-           "selection_mask": selection_mask, "n_selected": n, "n_isect": int(meta["flatten_ids"].numel())}
+           "selection_mask": selection_mask, "n_selected": n, "n_isect": int(meta["flatten_ids"].numel()),
+           "colors": colors, "alphas": alphas}
     if cls_id is not None and global_feat is not None:
         gv = torch.zeros(len(global_feat), dtype=torch.bool, device=dev)
         gv[cls_id[visible_mask].reshape(-1).long()] = True

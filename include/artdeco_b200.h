@@ -38,6 +38,37 @@ int adb_ssim_backward(int B, int CH, int H, int W, float C1, float C2, const flo
                       const float* dL_dmap, const float* dL_scalar, float dL_scale, const float* dm_dmu1,
                       const float* dm_dsigma1_sq, const float* dm_dsigma12, float* dL_dimg1, adb_stream_t stream);
 
+/* ---- mapper training loss (csrc/mapper_loss.cu) ----
+ * replaces the pixel loss block of SceneModel.optimization_step, Reconstruct/scene/scene_models/h3dgsv3.py:430-450, with
+ * render_from_id's exposure (:611-614) and render's background composite and 1/D (:682-686), and their autograd backward.
+ * One view of height h x width w.  colors [h,w,4] (RGB + accumulated depth D) and alphas [h,w] are the rasterizer's raw
+ * channels-last outputs (colors and v_colors 16-byte aligned); gt [3,h,w]; mono_idepth [h,w]; exposure [3,4]; bg [3];
+ * rdk [h,w] the radial weights (Reconstruct/utils.py:818-826).  Per pixel: c = rgb + (1 - alpha) bg,
+ * e = clamp(E[:, :3] c + E[:, 3], 0, 1), inv = 1/D and, when is_important == 0, the mask
+ * m = !(rdk|e0-g0| > 0.2 | rdk|e1-g1| > 0.2 | rdk|e1-g1| > 0.2) (as the reference writes it) multiplying e, gt, inv, mono.
+ * One workspace (adb_mapper_loss_workspace_bytes) serves a forward and its backward; the forward's partials stay in it
+ * until adb_mapper_loss_reduce.
+ *   adb_mapper_loss_forward   image [3,h,w] = m e and gt_masked [3,h,w] = m gt (the SSIM operands), invdepth [h,w] = m inv
+ *                             (may be NULL), and per-block partial sums of rdk|m e - m gt| and rdk|m inv - m mono|
+ *   adb_mapper_loss_reduce    after adb_ssim_forward(image, gt_masked) wrote ssim_map [3,h,w]: terms [4] = loss, l1, mean
+ *                             SSIM, depth term, with loss = lambda (1 - ssim) + (1 - lambda) l1 + depth_weight depth.
+ *                             Partials are added in a fixed order: bitwise reproducible
+ *   adb_mapper_loss_backward  dL [1] the upstream gradient of the loss (device); dssim [3,h,w] = adb_ssim_backward's
+ *                             dL/dimage called with dL_scalar = dL and dL_scale = -lambda / (3hw).  Writes v_colors [h,w,4],
+ *                             v_alphas [h,w] and v_exposure [3,4] (bg gets no gradient) */
+int adb_mapper_loss_workspace_bytes(int height, int width, size_t* bytes /*HOST*/);
+int adb_mapper_loss_forward(int height, int width, const float* colors, const float* alphas, const float* gt,
+                            const float* mono_idepth, const float* exposure, const float* bg, const float* rdk,
+                            int is_important, float* image, float* gt_masked, float* invdepth, void* ws, size_t ws_bytes,
+                            adb_stream_t stream);
+int adb_mapper_loss_reduce(int height, int width, const float* ssim_map, float lambda_dssim, float depth_weight,
+                           float* terms /*[4]*/, void* ws, size_t ws_bytes, adb_stream_t stream);
+int adb_mapper_loss_backward(int height, int width, const float* colors, const float* alphas, const float* gt,
+                             const float* mono_idepth, const float* exposure, const float* bg, const float* rdk,
+                             int is_important, const float* dssim, const float* dL, float lambda_dssim, float depth_weight,
+                             float* v_colors, float* v_alphas, float* v_exposure, void* ws, size_t ws_bytes,
+                             adb_stream_t stream);
+
 /* ---- Gaussian-splat rasterizer (one camera per call) ----
  * replaces the stages of gsplat.rendering.rasterization as called at
  * Reconstruct/scene/scene_models/h3dgsv3.py:664-680 (gsplat itself is an un-vendored pip dependency).
