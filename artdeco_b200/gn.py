@@ -22,7 +22,11 @@ _lib.register("adb_gauss_newton", [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, v
 
 
 def _solve(mode, Twc, Xs, Cs, K, ii, jj, idx_ii2jj, valid_match, Q, height, width, pixel_border, z_eps, sigma_a, sigma_b,
-           C_thresh, Q_thresh, max_iter, delta_thresh, return_state=False):
+           C_thresh, Q_thresh, max_iter, delta_thresh, return_state=False, return_workspace=False):
+    """Runs the solve.  Returns ``[dx]``, or a tuple that appends the device state [4] (``return_state``) and then the
+    uint8 workspace (``return_workspace``) in which the last iteration leaves, in this order: H [D,D] f64 (its strict
+    upper triangle still holds the assembled matrix, the lower triangle and the diagonal hold the Cholesky factor), b [D]
+    f64 (the solution x, dx = -x), S [E,28] f32 (lower triangle, row-major) and v [E,7] f32; D = 7 (K-1)."""
     _lib.require_cuda(Twc)
     dev = Twc.device
     if Twc.dim() != 2 or Twc.shape[1] != 8 or Twc.dtype != torch.float32:
@@ -31,8 +35,18 @@ def _solve(mode, Twc, Xs, Cs, K, ii, jj, idx_ii2jj, valid_match, Q, height, widt
     if Twc.shape[0] != Kp or Cs.shape[0] != Kp:
         raise ValueError("Twc, Xs and Cs must stack the same key frames")
     E = int(ii.shape[0])
+    if jj.shape[0] != E:
+        raise ValueError("ii and jj must list the same edges")
+    for name, t in (("idx_ii2jj", idx_ii2jj), ("valid_match", valid_match), ("Q", Q)):
+        if t.numel() != E * n:
+            raise ValueError(f"{name} must hold E*n = {E * n} elements, got {t.numel()}")
+    if mode == 1 and n != int(height) * int(width):
+        raise ValueError(f"calib mode needs one point per pixel: n = {n} but height*width = {int(height) * int(width)}")
     # gn_kernels.cu:160-171: unique sorted key-frame ids; edges address the pose table by their rank in it
     unique = torch.unique(torch.cat([ii, jj]), sorted=True)
+    if unique.numel() > Kp:
+        # a rank >= K would address a pose (and a pointmap) past the end of the tables
+        raise ValueError(f"the edges name {unique.numel()} key frames but Twc has {Kp} rows")
     ii_pos = torch.searchsorted(unique, ii.contiguous()).long().contiguous()
     jj_pos = torch.searchsorted(unique, jj.contiguous()).long().contiguous()
     poses = Twc if Twc.is_contiguous() else Twc.contiguous()
@@ -54,7 +68,9 @@ def _solve(mode, Twc, Xs, Cs, K, ii, jj, idx_ii2jj, valid_match, Q, height, widt
                   float(delta_thresh), _lib.ptr(dx), _lib.ptr(state), _lib.ptr(ws), ws.numel(), _lib.stream())
     if poses is not Twc:
         Twc.copy_(poses)
-    return ([dx], state) if return_state else [dx]
+    if not (return_state or return_workspace):
+        return [dx]
+    return ([dx],) + ((state,) if return_state else ()) + ((ws,) if return_workspace else ())
 
 
 def gauss_newton_rays(Twc, Xs, Cs, ii, jj, idx_ii2jj, valid_match, Q, sigma_ray, sigma_dist, C_thresh, Q_thresh, max_iter,

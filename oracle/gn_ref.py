@@ -2,7 +2,8 @@
 and host loop restated in PyTorch — residuals, Huber weights, Jacobians (gn_kernels.cu:924-1095 rays, :1346-1500 calib),
 ``apply_Sim3_adj_inv`` (:267-290), the 14x14 block layout and the index bookkeeping of ``SparseBlock`` (:71-113), a double
 Cholesky solve (the reference: Eigen SimplicialLLT in double, :136-160), ``expSim3`` / ``retrSim3`` (:316-412) and the
-termination rule of the host loop (:1141-1229).  Everything except the solve runs in float32 like the kernels.
+termination rule of the host loop (:1141-1229).  By default everything except the solve runs in float32 like the kernels;
+``dtype=torch.float64`` gives the high-precision run the tests compare the kernels' stages with.
 PARITY UNPINNED by the reference: its GN extension needs Eigen, which is not vendored, so it cannot be built here; this is a
 restatement from the source."""
 import torch
@@ -26,7 +27,7 @@ def act_so3(q, X):
 
 def rel_sim3(ti, qi, si, tj, qj, sj):
     si_inv = 1.0 / si
-    qi_inv = qi * torch.tensor([-1.0, -1.0, -1.0, 1.0], dtype=qi.dtype)
+    qi_inv = qi * torch.tensor([-1.0, -1.0, -1.0, 1.0], dtype=qi.dtype, device=qi.device)
     return act_so3(qi_inv, tj - ti) * si_inv, quat_comp(qi_inv, qj), si_inv * sj
 
 
@@ -56,7 +57,7 @@ def _rows_rays(P, Xi, valid, q, sigma_ray, sigma_dist):
     sw = torch.stack([sw_a, sw_a, sw_a, sw_b], -1)
     w = huber(sw * err) * sw * sw
     n3 = 1.0 / (n1j * n2j)
-    eye = torch.eye(3, dtype=P.dtype)
+    eye = torch.eye(3, dtype=P.dtype, device=P.device)
     dr = eye / n1j[..., None] - P[..., :, None] * P[..., None, :] * n3[..., None]   # [n,3,3]
     z = torch.zeros_like(r[..., 0])
     rot = torch.stack([torch.stack([z, r[..., 2], -r[..., 1]], -1), torch.stack([-r[..., 2], z, r[..., 0]], -1),
@@ -110,7 +111,7 @@ def exp_sim3(xi):
     q = exp_so3(phi)
     th2 = (phi * phi).sum()
     th = th2.sqrt()
-    one = torch.tensor(1.0, dtype=xi.dtype)
+    one = torch.tensor(1.0, dtype=xi.dtype, device=xi.device)
     if sigma.abs() < EPS:
         C = one
         if th.abs() < EPS:
@@ -132,59 +133,156 @@ def exp_sim3(xi):
     return C * tau + A * c1 + B * c2, q, scale
 
 
-def gauss_newton(mode, Twc, Xs, Cs, ii, jj, idx_ii2jj, valid_match, Q, sigma_a, sigma_b, C_thresh, Q_thresh, max_iter,
-                 delta_thresh, K=None, height=0, width=0, pixel_border=0, z_eps=0.0):
-    """mode 'rays' | 'calib'.  Twc [K,8] float32 is updated in place; returns (dx_last [K-1,7], iterations run)."""
-    num_fix = 1
-    E, n = idx_ii2jj.shape[0], Xs.shape[1]
+HUBER_K = 1.345
+
+
+def _rel_margin(x, t):
+    """|x - t| relative to the larger operand: how far a gated value is from flipping its decision."""
+    t = torch.as_tensor(t, dtype=x.dtype, device=x.device)
+    return (x - t).abs() / torch.maximum(x.abs(), t.abs()).clamp_min(1e-30)
+
+
+def edge_ranks(ii, jj):
+    """Key-frame ids -> positions in the pose table (the rank of the id among the unique sorted ids, gn_kernels.cu:160-171)."""
     unique = torch.unique(torch.cat([ii, jj]), sorted=True)
-    ie, je = torch.searchsorted(unique, ii), torch.searchsorted(unique, jj)
+    return torch.searchsorted(unique, ii), torch.searchsorted(unique, jj)
+
+
+def edge_blocks(mode, Twc, Xs, Cs, ii, jj, idx_ii2jj, valid_match, Q, sigma_a, sigma_b, C_thresh, Q_thresh, K=None, height=0,
+                width=0, pixel_border=0, z_eps=0.0, dtype=torch.float32, return_rows=False):
+    """The per-edge normal-equation blocks of one iteration, computed in ``dtype``.
+
+    Returns a dict:
+      S [E,7,7], v [E,7]  the j-side block sum_n w J J^T and gradient sum_n w e J (the i side is the negation: Ji = -Jj);
+      A [E,7,7], B [E,7]  magnitude sums  sum w' |J_a||J_b|  and  sum w (|e| + u_e) |J_a|, where u_e is the size of the
+                          operands whose difference forms the residual (1 for the unit-ray components, |P| for the distance,
+                          the pixel coordinate plus the principal point for u / v, 1 + |log z| for the log depth): rounding
+                          in an fp32 evaluation scales with these, so they set the tolerance of a comparison; w' adds
+                          w u_e / |e| where huber is active (w = 1.345 sw / |e| inherits the rounding of e);
+      margin_pt [E,n]     per point, the smallest relative distance of a gated value to its threshold (Q_thresh, the two
+                          confidences against C_thresh, huber's 1.345; calib also z_eps for P_z and Xi_z and the four
+                          pixel-border limits); +inf where valid_match is false;
+      margin              its minimum;
+      err, w, J           (return_rows) the residual rows [E,n,R], their weights and the j-side Jacobian rows [E,n,R,7].
+    ``ii`` / ``jj`` are key-frame ids, mapped to pose-table positions as the reference does."""
+    E, n, Kp = idx_ii2jj.shape[0], Xs.shape[1], Xs.shape[0]
+    ie, je = edge_ranks(ii, jj)
+    T, X = Twc.to(dtype), Xs.to(dtype)
+    Cs2, Q2 = Cs.reshape(Kp, n).to(dtype), Q.reshape(E, n).to(dtype)
+    vm2, idx2 = valid_match.reshape(E, n).bool(), idx_ii2jj.reshape(E, n).long()
+    Kd = K.to(dtype) if K is not None else None
+    R = 4 if mode == "rays" else 3
+    out = {k: [] for k in ("S", "v", "A", "B", "margin_pt", "err", "w", "J")}
+    step = max(1, (1 << 17) // max(n, 1))                                  # edges per batch
+    for e0 in range(0, E, step):
+        sl = slice(e0, min(E, e0 + step))
+        ix, jx = ie[sl], je[sl]
+        ti, qi, si = T[ix, None, 0:3], T[ix, None, 3:7], T[ix, None, 7:8]     # [e,1,.]
+        tj, qj, sj = T[jx, None, 0:3], T[jx, None, 3:7], T[jx, None, 7:8]
+        tij, qij, sij = rel_sim3(ti, qi, si, tj, qj, sj)
+        vm = vm2[sl]
+        ind = torch.where(vm, idx2[sl], torch.zeros_like(idx2[sl]))
+        Xi = torch.gather(X[ix], 1, ind[..., None].expand(-1, -1, 3))
+        Xj = X[jx]
+        P = act_so3(qij.expand(Xj.shape[:-1] + (4,)), Xj) * sij + tij
+        q = Q2[sl]
+        ci, cj = torch.gather(Cs2[ix], 1, ind), Cs2[jx]
+        valid = vm & (q > Q_thresh) & (ci > C_thresh) & (cj > C_thresh)
+        gates = [_rel_margin(q, Q_thresh), _rel_margin(ci, C_thresh), _rel_margin(cj, C_thresh)]
+        if mode == "rays":
+            err, w, Jrow = _rows_rays(P, Xi, valid, q, sigma_a, sigma_b)
+            n1 = torch.maximum(P.norm(dim=-1), Xi.norm(dim=-1))
+            ue = torch.stack([torch.ones_like(n1)] * 3 + [n1], -1)
+            sw = torch.stack([q.sqrt() / sigma_a] * 3 + [q.sqrt() / sigma_b], -1)
+        else:
+            err, w, Jrow = _rows_calib(P, Xi, ind, valid, q, Kd, height, width, pixel_border, z_eps, sigma_a, sigma_b)
+            fx, fy, cx, cy = Kd[0, 0], Kd[1, 1], Kd[0, 2], Kd[1, 2]
+            vz = (P[..., 2] > z_eps) & (Xi[..., 2] > z_eps)
+            zi = torch.where(vz, 1.0 / P[..., 2], torch.zeros_like(P[..., 2]))
+            u, vv = fx * P[..., 0] * zi + cx, fy * P[..., 1] * zi + cy
+            u_t, v_t = (ind % width).to(dtype), (ind // width).to(dtype)
+            lz = torch.maximum(P[..., 2].abs().clamp_min(1e-30).log().abs(), Xi[..., 2].abs().clamp_min(1e-30).log().abs())
+            ue = torch.stack([torch.maximum(u.abs(), u_t) + cx.abs(), torch.maximum(vv.abs(), v_t) + cy.abs(), 1.0 + lz], -1)
+            sw = torch.stack([q.sqrt() / sigma_a] * 2 + [q.sqrt() / sigma_b], -1)
+            gates += [_rel_margin(P[..., 2], z_eps), _rel_margin(Xi[..., 2], z_eps),
+                      _rel_margin(u, pixel_border), _rel_margin(u, width - 1 - pixel_border),
+                      _rel_margin(vv, pixel_border), _rel_margin(vv, height - 1 - pixel_border)]
+        # huber's switch only matters where the point is used (its weight is continuous there anyway)
+        hub = torch.where(valid[..., None], _rel_margin((sw * err).abs(), HUBER_K), torch.full_like(err, float("inf")))
+        gates.append(hub.amin(-1))
+        m = torch.stack(gates, -1).amin(-1)
+        out["margin_pt"].append(torch.where(vm, m, torch.full_like(m, float("inf"))))
+        Jj = adj_inv(ti[:, :, None], qi[:, :, None], si[:, :, None], Jrow)      # [e,n,R,7]
+        aJ = Jj.abs()
+        # where huber is active w = 1.345 sw / |e|: its rounding is that of e, relative u_e / |e|
+        active = (sw * err).abs() >= HUBER_K
+        wA = w * (1.0 + torch.where(active, ue / err.abs().clamp_min(1e-30), torch.zeros_like(ue)))
+        out["S"].append(torch.einsum("enr,enra,enrb->eab", w, Jj, Jj))
+        out["v"].append(torch.einsum("enr,enr,enra->ea", w, err, Jj))
+        out["A"].append(torch.einsum("enr,enra,enrb->eab", wA, aJ, aJ))
+        out["B"].append(torch.einsum("enr,enr,enra->ea", w, err.abs() + ue, aJ))
+        if return_rows:
+            out["err"].append(err)
+            out["w"].append(w)
+            out["J"].append(Jj)
+    res = {k: torch.cat(vs) if vs else torch.zeros(0) for k, vs in out.items()}
+    res["margin"] = float(res["margin_pt"].min()) if res["margin_pt"].numel() else float("inf")
+    if not return_rows:
+        for k in ("err", "w", "J"):
+            res.pop(k)
+    return res
+
+
+def assemble(S, v, ie, je, n_poses, num_fix=1):
+    """The dense system of the free poses in float64: block (i,i) += S, (j,j) += S, (i,j) = (j,i) -= S, b_i -= v, b_j += v;
+    rows and columns of the fixed poses are dropped (SparseBlock::update_lhs / update_rhs, gn_kernels.cu:71-113)."""
+    D = 7 * (n_poses - num_fix)
+    H = torch.zeros(D, D, dtype=torch.float64)
+    b = torch.zeros(D, dtype=torch.float64)
+    S, v = S.double().cpu(), v.double().cpu()
+    for e in range(S.shape[0]):
+        io, jo = int(ie[e]) - num_fix, int(je[e]) - num_fix
+        for (a, sa) in ((io, -1.0), (jo, 1.0)):
+            if a < 0:
+                continue
+            b[a * 7:a * 7 + 7] += sa * v[e]
+            for (c, sc) in ((io, -1.0), (jo, 1.0)):
+                if c >= 0:
+                    H[a * 7:a * 7 + 7, c * 7:c * 7 + 7] += (sa * sc) * S[e]
+    return H, b
+
+
+def retract(Twc, dx, num_fix=1):
+    """Twc[k] <- exp(dx[k - num_fix]) Twc[k] for the free poses, in the dtype of ``dx`` (retrSim3, gn_kernels.cu:387-412)."""
+    for k in range(num_fix, Twc.shape[0]):
+        dt, dq, ds = exp_sim3(dx[k - num_fix])
+        t, q, s = Twc[k, 0:3].clone(), Twc[k, 3:7].clone(), Twc[k, 7].clone()
+        Twc[k, 3:7] = quat_comp(dq, q)
+        Twc[k, 0:3] = act_so3(dq, t) * ds + dt
+        Twc[k, 7] = ds * s
+    return Twc
+
+
+def gauss_newton(mode, Twc, Xs, Cs, ii, jj, idx_ii2jj, valid_match, Q, sigma_a, sigma_b, C_thresh, Q_thresh, max_iter,
+                 delta_thresh, K=None, height=0, width=0, pixel_border=0, z_eps=0.0, dtype=torch.float32):
+    """mode 'rays' | 'calib'.  Twc [K,8] is updated in place; returns (dx_last [K-1,7], iterations run).  The blocks, the
+    step and the retraction are evaluated in ``dtype`` (float32 like the kernels, float64 for a high-precision run); the
+    system is always assembled and solved in double."""
+    num_fix = 1
     Kp = Xs.shape[0]
-    D = 7 * (Kp - num_fix)
-    Cs2, Q2, vm2 = Cs.reshape(Kp, n), Q.reshape(E, n), valid_match.reshape(E, n)
-    dx, its = torch.zeros(Kp - num_fix, 7), 0
+    ie, je = edge_ranks(ii.cpu(), jj.cpu())
+    dx, its = torch.zeros(Kp - num_fix, 7, dtype=dtype, device=Twc.device), 0
     for _ in range(max_iter):
-        H = torch.zeros(D, D, dtype=torch.float64)
-        b = torch.zeros(D, dtype=torch.float64)
-        for e in range(E):
-            ix, jx = int(ie[e]), int(je[e])
-            ti, qi, si = Twc[ix, 0:3], Twc[ix, 3:7], Twc[ix, 7:8]
-            tj, qj, sj = Twc[jx, 0:3], Twc[jx, 3:7], Twc[jx, 7:8]
-            tij, qij, sij = rel_sim3(ti, qi, si, tj, qj, sj)
-            vm = vm2[e]
-            ind = torch.where(vm, idx_ii2jj[e], torch.zeros_like(idx_ii2jj[e]))
-            Xi, Xj = Xs[ix][ind], Xs[jx]
-            P = act_so3(qij, Xj) * sij + tij
-            q = Q2[e]
-            valid = vm & (q > Q_thresh) & (Cs2[ix][ind] > C_thresh) & (Cs2[jx] > C_thresh)
-            if mode == "rays":
-                err, w, Jrow = _rows_rays(P, Xi, valid, q, sigma_a, sigma_b)
-            else:
-                err, w, Jrow = _rows_calib(P, Xi, ind, valid, q, K, height, width, pixel_border, z_eps, sigma_a, sigma_b)
-            Jj = adj_inv(ti, qi, si, Jrow)                                  # [n,R,7]
-            Jx = torch.cat([-Jj, Jj], -1)                                    # Ji = -Jj
-            Hb = torch.einsum("nr,nra,nrb->ab", w, Jx, Jx).double()          # fp32 products, like the kernel
-            g = torch.einsum("nr,nr,nra->a", w, err, Jx).double()
-            io, jo = ix - num_fix, jx - num_fix
-            for (a, ra) in ((io, 0), (jo, 7)):
-                if a < 0:
-                    continue
-                b[a * 7:a * 7 + 7] += g[ra:ra + 7]
-                for (c, rc) in ((io, 0), (jo, 7)):
-                    if c >= 0:
-                        H[a * 7:a * 7 + 7, c * 7:c * 7 + 7] += Hb[ra:ra + 7, rc:rc + 7]
+        blk = edge_blocks(mode, Twc, Xs, Cs, ii, jj, idx_ii2jj, valid_match, Q, sigma_a, sigma_b, C_thresh, Q_thresh, K=K,
+                          height=height, width=width, pixel_border=pixel_border, z_eps=z_eps, dtype=dtype)
+        H, b = assemble(blk["S"], blk["v"], ie, je, Kp, num_fix)
         try:
             L = torch.linalg.cholesky(H)
             x = torch.cholesky_solve(b[:, None], L)[:, 0]
-            dx = (-x).float().reshape(-1, 7)
+            dx = (-x).to(dtype).reshape(-1, 7).to(Twc.device)
         except Exception:  # noqa: BLE001  (SimplicialLLT failure path returns zeros)
-            dx = torch.zeros(Kp - num_fix, 7)
-        for k in range(num_fix, Kp):
-            dt, dq, ds = exp_sim3(dx[k - num_fix])
-            t, q, s = Twc[k, 0:3].clone(), Twc[k, 3:7].clone(), Twc[k, 7].clone()
-            Twc[k, 3:7] = quat_comp(dq, q)
-            Twc[k, 0:3] = act_so3(dq, t) * ds + dt
-            Twc[k, 7] = ds * s
+            dx = torch.zeros(Kp - num_fix, 7, dtype=dtype, device=Twc.device)
+        retract(Twc, dx, num_fix)
         its += 1
         if float(dx.norm()) < delta_thresh:
             break
