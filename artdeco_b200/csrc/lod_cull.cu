@@ -28,7 +28,9 @@ lod_mask_kernel(long long N, const float* __restrict__ xyz, const float* __restr
 
 // weed_out_gaussians (h3dgsv3.py:942-953): the reference loops over every key frame in Python and streams all N rows once per
 // key frame (K x ~6 torch kernels).  Here one pass over the 16 B/Gaussian counts the key frames that see each Gaussian
-// (camera centres staged in shared memory) and applies the keep rule  count / K > visible_threshold  in fp32 as torch does.
+// (camera centres staged in shared memory) and applies the keep rule  count / K > visible_threshold  in fp32 as torch does
+// on the device: an int tensor over a Python int is count * fl32(1 / K), which differs from a correctly rounded division at
+// some counts (K = 500, count = 5 at threshold 0.01: the reference keeps that Gaussian).
 constexpr int WEED_MAX_CAMS_SMEM = 1024;
 __global__ void __launch_bounds__(256)
 weed_out_kernel(long long N, const float* __restrict__ xyz, const float* __restrict__ d_max, int K,
@@ -51,7 +53,7 @@ weed_out_kernel(long long N, const float* __restrict__ xyz, const float* __restr
     }
     if (i < N) {
         if (visible_count) visible_count[i] = cnt;
-        keep[i] = ((float)cnt / (float)K > visible_threshold) ? 1 : 0;
+        keep[i] = (__fmul_rn((float)cnt, __fdiv_rn(1.0f, (float)K)) > visible_threshold) ? 1 : 0;
     }
 }
 

@@ -45,12 +45,16 @@ __device__ __forceinline__ unsigned table_find(const u64* __restrict__ keys, uns
     }
 }
 
-__device__ __forceinline__ u64 voxel_key(const float* __restrict__ p, long long i, const float* __restrict__ mn, float voxel,
+// torch: floor((p - min) / voxel_size).long() with a Python-float voxel_size, which PyTorch's CUDA kernel evaluates as
+// (p - min) * fl32(1 / voxel_size).  A correctly rounded division puts some points in the neighbouring voxel
+// (1.3f / 0.1f = 12.999999, 1.3f * fl32(1 / 0.1f) = 13), so the reciprocal is taken once and multiplied, without contraction.
+__device__ __forceinline__ float voxel_inv(float voxel) { return __fdiv_rn(1.0f, voxel); }
+
+__device__ __forceinline__ u64 voxel_key(const float* __restrict__ p, long long i, const float* __restrict__ mn, float inv,
                                          int* __restrict__ overflow) {
-    // torch: floor((p - min) / voxel_size).long()
-    const long long vx = (long long)floorf((p[3 * i] - mn[0]) / voxel);
-    const long long vy = (long long)floorf((p[3 * i + 1] - mn[1]) / voxel);
-    const long long vz = (long long)floorf((p[3 * i + 2] - mn[2]) / voxel);
+    const long long vx = (long long)floorf(__fmul_rn(__fsub_rn(p[3 * i], mn[0]), inv));
+    const long long vy = (long long)floorf(__fmul_rn(__fsub_rn(p[3 * i + 1], mn[1]), inv));
+    const long long vz = (long long)floorf(__fmul_rn(__fsub_rn(p[3 * i + 2], mn[2]), inv));
     if ((vx | vy | vz) >> 21) *overflow = 1;
     return ((u64)vx << 42) | ((u64)vy << 21) | (u64)vz;
 }
@@ -61,7 +65,7 @@ voxel_insert_orig_kernel(long long N, const float* __restrict__ xyz, const long 
                          unsigned pmask, unsigned* __restrict__ slot_of, int* __restrict__ overflow) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N) return;
-    const u64 key = voxel_key(xyz, i, mn, voxel, overflow);
+    const u64 key = voxel_key(xyz, i, mn, voxel_inv(voxel), overflow);
     const unsigned s = table_insert(vkeys, vmask, key);
     slot_of[i] = s;
     const u64 pair = ((u64)s << 32) | (u64)(unsigned)cls[i];
@@ -95,7 +99,7 @@ voxel_match_new_kernel(long long M, const float* __restrict__ xyz, const float* 
                        int* __restrict__ overflow) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= M) return;
-    const u64 key = voxel_key(xyz, i, mn, voxel, overflow);
+    const u64 key = voxel_key(xyz, i, mn, voxel_inv(voxel), overflow);
     const unsigned s = have_orig ? table_find(vkeys, vmask, key) : 0xffffffffu;
     if (s != 0xffffffffu) {
         out[i] = (long long)(0xffffffffu - (unsigned)best[s]);

@@ -26,6 +26,15 @@ def _pow2(n: int) -> int:
     return p
 
 
+def max_class_id(cls: torch.Tensor) -> int:
+    """The largest class id (one host sync, like the reference's own ``max().item()``).  The kernels carry class ids as
+    32-bit values (the vote packs ``count << 32 | 0xffffffff - id``), so an id at or above 2^32 - 1 is refused."""
+    m = int(cls.max().item())
+    if m >= 0xFFFFFFFF:
+        raise _lib.ArtdecoB200Error(f"update_voxel: class id {m} does not fit the kernels' 32-bit ids (must be < 2^32 - 1)")
+    return m
+
+
 @torch.no_grad()
 def update_voxel(new_xyz: torch.Tensor, xyz: torch.Tensor, cls_id: torch.Tensor, voxel_size: float = 0.1):
     """Returns ``(updated_orig_cls_id [N,1] int64, updated_new_cls_id [M,1] int64, new_voxel_count)``; with no original points
@@ -46,7 +55,7 @@ def update_voxel(new_xyz: torch.Tensor, xyz: torch.Tensor, cls_id: torch.Tensor,
             xyz_c = xyz.detach().float().contiguous()
             cls = cls_id.detach().reshape(-1).long().contiguous()
             mn = (torch.minimum(xyz_c.amin(0), new_c.amin(0)) if M > 0 else xyz_c.amin(0)).contiguous()
-            max_cls = int(cls.max().item())                      # the reference syncs here too (h3dgsv3.py:260)
+            max_cls = max_class_id(cls)                          # the reference syncs here too (h3dgsv3.py:260)
             V = P = _pow2(2 * N)
             vkeys = torch.full((V,), -1, dtype=torch.int64, device=dev)
             pkeys = torch.full((P,), -1, dtype=torch.int64, device=dev)

@@ -353,6 +353,8 @@ int adb_track_finish(int height, int width, const long long* idx_f2k, const unsi
 /* update_voxel (Reconstruct/scene/scene_models/h3dgsv3.py:227-316): voxel-hash class ids without the reference's three sorts
  * (csrc/voxel.cu).  Tables are caller-allocated: vkeys[V], pkeys[P], ukeys[U] uint64 pre-filled with 0xFF bytes; pcount[P]
  * int32 and best[V] uint64 zeroed; V, P powers of two >= 2N, U >= 2M.  mn = device float[3] minimum over all points.
+ * Voxel index floor((p - mn) * fp32(1 / voxel_size)), PyTorch's device arithmetic for the reference's division; class ids
+ * are read as 32-bit unsigned values.
  *   adb_voxel_vote       original points -> cls_out[N] = majority class of each point's voxel (ties: smallest id)
  *   adb_voxel_match_new  new points: voxel's class, or their voxel key collected into ulist (count in *ucount, device)
  *   adb_voxel_rank_new   `sorted` = the distinct unmatched keys ascending (caller sorts) -> cls_out = base + rank */
@@ -365,7 +367,8 @@ int adb_voxel_match_new(long long M, const float* new_xyz, const float* mn, floa
 int adb_voxel_rank_new(long long M, int n, const void* sorted, const void* ukeys, long long U, int* urank,
                        const int* uslot_of, long long base, long long* cls_out, adb_stream_t stream);
 /* weed_out_gaussians (Reconstruct/scene/scene_models/h3dgsv3.py:942-953) for ALL key frames in one pass: cams [K,3] camera
- * centres (device); keep[i] = (#{k : |xyz_i - cam_k| < 2 d_max_i} / K > visible_threshold); visible_count [N] may be NULL. */
+ * centres (device); keep[i] = (count_i * fp32(1 / K) > visible_threshold) with count_i = #{k : |xyz_i - cam_k| < 2 d_max_i},
+ * PyTorch's device arithmetic for the reference's count / K; visible_count [N] may be NULL. */
 /* Key-frame densification: the sampler of SceneModel.add_new_gaussians (Reconstruct/scene/scene_models/h3dgsv3.py:766-940,
  * csrc/densify.cu).  One workspace (adb_densify_workspace_bytes for the LoD-1 image, height x width) serves every call.
  *   adb_densify_depth_quantile  out[0] = torch.quantile(values[n], q) (linear, NaN if any value is NaN),

@@ -7,6 +7,7 @@ h3dgsv3.py:766-940 with the helpers of Reconstruct/utils.py:93-108, :119-130, :1
   * ``update_voxel`` defaults to ``oracle.voxel_ref.update_voxel`` (run on the CPU) and may be replaced;
   * ``weed_out_gaussians`` takes the key frames' centres ``keyframe.get_Rt().T.inverse()[3, :3]``.
 PARITY: pinned against the reference's own code by tests/golden/make_densify_golden.py (tests/golden/densify_small.pt)."""
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -189,5 +190,8 @@ def weed_out(params, cam_centres, visible_threshold):
     for c in cam_centres:
         dist = (xyz - c).norm(dim=1, keepdim=True)
         count += (dist < 2 * params["d_max"]).squeeze(-1).int()
-    mask = (count / len(cam_centres)) > visible_threshold
+    # the reference's count / len(keyframes) on a CUDA tensor is count * fl32(1 / K) (PyTorch's CPU-scalar fast path);
+    # written out so that the oracle gives that answer on the CPU as well
+    inv = torch.tensor(np.float32(1.0) / np.float32(len(cam_centres)), device=count.device)
+    mask = (count.float() * inv) > visible_threshold
     add_and_prune(params, {k: v[:0] for k, v in params.items()}, mask)

@@ -119,7 +119,9 @@ def test_lod_select_matches_reference_formula(cuda, N):
 @pytest.mark.parametrize("N,K", [(1, 1), (50_000, 7), (200_000, 40)])
 def test_weed_out_mask_matches_the_reference_loop(cuda, N, K):
     """weed_out_gaussians (h3dgsv3.py:942-953) restated line for line with torch on the CPU (the per-key-frame loop IS the
-    reference code path) against the one-pass kernel; the same fp32 strict-'<' caveat as the LoD select applies."""
+    reference code path) against the one-pass kernel; the same fp32 strict-'<' caveat as the LoD select applies.  The
+    keep rule is written as the device computes the reference's count / K (times the fp32 reciprocal of K): CPU torch
+    divides."""
     from artdeco_b200.cull import weed_out_mask
     sc = synthetic.raster_scene(N, seed=5)
     xyz, d_max = sc["means"], sc["d_max"] * 0.2
@@ -130,7 +132,7 @@ def test_weed_out_mask_matches_the_reference_loop(cuda, N, K):
     for k in range(K):
         ob_dist = (xyz - cams[k]).norm(dim=1, keepdim=True)
         visible_count += (ob_dist < 2 * d_max).squeeze(-1).int()
-    weed = (visible_count / K) > thr
+    weed = (visible_count.float() * torch.tensor(np.float32(1.0) / np.float32(K))) > thr
     keep, cnt = weed_out_mask(xyz.to(cuda), d_max.to(cuda), cams.to(cuda), thr, return_count=True)
     dc = (cnt.cpu() != visible_count)
     assert dc.sum() <= max(2, N * K // 100000), "visible counts (last-ulp distance ties only)"
