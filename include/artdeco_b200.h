@@ -69,6 +69,32 @@ int adb_mapper_loss_backward(int height, int width, const float* colors, const f
                              float* v_colors, float* v_alphas, float* v_exposure, void* ws, size_t ws_bytes,
                              adb_stream_t stream);
 
+/* ---- map re-anchoring after the Backend moves its key frames (csrc/reanchor.cu) ----
+ *   adb_reanchor_keyframes  replaces the pose loop of run_system.py:194-226 (pypose SE3 / quat2unit / mul / Inv / matrix,
+ *                           Keyframe.get_Rt / set_Rt, three torch.linalg.inv per mapper key frame) for all K frames in one
+ *                           launch.  slam_T_WC [K_slam,8] the Backend's Sim(3) table (tx ty tz qx qy qz qw s);
+ *                           last_keyframe_index [K] int64, is_slam_keyframe [K] uint8, T_CkCf [K,8] (read on non-SLAM rows
+ *                           only); rW2C [K,3,2] / tW2C [K,3] updated IN PLACE (set_Rt).  Writes old_c2w / new_c2w [K,4,4]
+ *                           (the inverses of get_Rt before and of new_Rt), approx_centres [K,3] = -new_R^T t and
+ *                           cam_centres [K,3] = inverse(get_Rt().T)[3,:3] after set_Rt (sixD2mtx's re-orthonormalised R).
+ *                           A row whose index is outside [0, K_slam) keeps its pose (new_c2w = old_c2w, both centres its
+ *                           current one) and adds 1 to *n_bad (device int32, caller-zeroed)
+ *   adb_reanchor_gaussians  replaces SceneModel.rigid_transform_gs (Reconstruct/scene/scene_models/h3dgsv3.py:955-966) and
+ *                           update_gaussians (Reconstruct/utils.py:28-60): per Gaussian, with D = new_c2w[id] inv(old_c2w[id]),
+ *                           xyz_out = D[:3,:3] xyz + D[:3,3] and rotation_out = mat2quat(D[:3,:3] quat2mat(rotation)) with
+ *                           kornia's conversions (wxyz).  ids [N] int64, xyz [N,3], rotation [N,4]; rotation, rotation_out
+ *                           and ws 16-byte aligned; outputs must not overlap inputs.  Rows with an id outside [0, K) or a
+ *                           singular old_c2w[id] (zero pivot) are copied unchanged and added to *n_bad.  Two launches (one
+ *                           over K, one over N); N == 0 launches nothing.  ws: adb_reanchor_workspace_bytes(K) */
+int adb_reanchor_workspace_bytes(int K, size_t* bytes /*HOST*/);
+int adb_reanchor_keyframes(int K, int K_slam, const float* slam_T_WC, const long long* last_keyframe_index,
+                           const unsigned char* is_slam_keyframe, const float* T_CkCf, float* rW2C, float* tW2C,
+                           float* old_c2w, float* new_c2w, float* cam_centres, float* approx_centres, int32_t* n_bad,
+                           adb_stream_t stream);
+int adb_reanchor_gaussians(long long N, int K, const long long* ids, const float* xyz, const float* rotation,
+                           const float* old_c2w, const float* new_c2w, float* xyz_out, float* rotation_out, int32_t* n_bad,
+                           void* ws, size_t ws_bytes, adb_stream_t stream);
+
 /* ---- Gaussian-splat rasterizer (one camera per call) ----
  * replaces the stages of gsplat.rendering.rasterization as called at
  * Reconstruct/scene/scene_models/h3dgsv3.py:664-680 (gsplat itself is an un-vendored pip dependency).
