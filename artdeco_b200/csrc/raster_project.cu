@@ -5,45 +5,13 @@
 // Reconstruct/scene/scene_models/h3dgsv3.py:664-680: the projection (SURVEY.md App. B.1), the degree-3 SH
 // evaluation with the +0.5 / clamp (App. B.2) and the tile count of isect_tiles (App. B.3).  gsplat runs
 // these as three kernels with [N]-sized round trips through HBM between them; here one thread per
-// Gaussian reads the 236 B of parameters once and writes one 48 B splat record + radii + count.
-#include "raster_common.cuh"
+// Gaussian reads the 236 B of parameters once and writes one 48 B splat record + radii + count.  The projection and SH
+// math shared with the backward kernels is in raster_geom.cuh.
+#include "raster_geom.cuh"
 #include "adb_detmath.h"
 #include <stdio.h>
 
 namespace {
-
-__device__ __forceinline__ void mat3_mul(const float* A, const float* B, float* C) {
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j)
-            C[i * 3 + j] = A[i * 3 + 0] * B[0 * 3 + j] + A[i * 3 + 1] * B[1 * 3 + j] + A[i * 3 + 2] * B[2 * 3 + j];
-}
-__device__ __forceinline__ void mat3_mul_bt(const float* A, const float* B, float* C) {
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j)
-            C[i * 3 + j] = A[i * 3 + 0] * B[j * 3 + 0] + A[i * 3 + 1] * B[j * 3 + 1] + A[i * 3 + 2] * B[j * 3 + 2];
-}
-
-__device__ __forceinline__ void sh_basis(int deg, float x, float y, float z, float* B) {
-#pragma unroll
-    for (int k = 0; k < 16; ++k) B[k] = 0.f;
-    B[0] = 0.2820947917738781f;
-    if (deg < 1) return;
-    B[1] = -0.48860251190292f * y; B[2] = 0.48860251190292f * z; B[3] = -0.48860251190292f * x;
-    if (deg < 2) return;
-    float z2 = z * z, fT0B = -1.092548430592079f * z, fC1 = x * x - y * y, fS1 = 2.f * x * y;
-    B[4] = 0.5462742152960395f * fS1; B[5] = fT0B * y; B[6] = 0.9461746957575601f * z2 - 0.3153915652525201f;
-    B[7] = fT0B * x; B[8] = 0.5462742152960395f * fC1;
-    if (deg < 3) return;
-    float fT0C = -2.285228997322329f * z2 + 0.4570457994644658f, fT1B = 1.445305721320277f * z;
-    float fC2 = x * fC1 - y * fS1, fS2 = x * fS1 + y * fC1;
-    B[9] = -0.5900435899266435f * fS2; B[10] = fT1B * fS1; B[11] = fT0C * y;
-    B[12] = z * (1.865881662950577f * z2 - 1.119528997770346f); B[13] = fT0C * x; B[14] = fT1B * fC1;
-    B[15] = -0.5900435899266435f * fC2;
-}
 
 // C cameras (viewmat / K / campos point at [C,16] / [C,9] / [C,3]); outputs are [C,N,...] stacks and tile_counts holds C
 // consecutive counter blocks of 2 * COPIES * T.  Work split: warp w of the grid handles view (w % C) of the 32 Gaussians of
@@ -86,37 +54,18 @@ project_fwd_kernel(int N, int C, const float* __restrict__ means, const float* _
     if (ok) {
         float Rq[9];
         {
-            float4 q = reinterpret_cast<const float4*>(quats)[i];
-            float w = q.x, qx = q.y, qy = q.z, qz = q.w;
-            float n2 = w * w + qx * qx + qy * qy + qz * qz;
-            float inv = 1.0f / sqrtf(n2);
-            w = w * inv; qx = qx * inv; qy = qy * inv; qz = qz * inv;
-            float x2 = qx * qx, y2 = qy * qy, z2 = qz * qz;
-            float xy = qx * qy, xz = qx * qz, yz = qy * qz, wx = w * qx, wy = w * qy, wz = w * qz;
-            Rq[0] = 1.0f - 2.0f * (y2 + z2); Rq[1] = 2.0f * (xy - wz);        Rq[2] = 2.0f * (xz + wy);
-            Rq[3] = 2.0f * (xy + wz);        Rq[4] = 1.0f - 2.0f * (x2 + z2); Rq[5] = 2.0f * (yz - wx);
-            Rq[6] = 2.0f * (xz - wy);        Rq[7] = 2.0f * (yz + wx);        Rq[8] = 1.0f - 2.0f * (x2 + y2);
+            const float4 q = reinterpret_cast<const float4*>(quats)[i];
+            const float inv = 1.0f / sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w);
+            quat_to_rotmat(q.x * inv, q.y * inv, q.z * inv, q.w * inv, Rq);
         }
         const float s[3] = {scales[3 * i], scales[3 * i + 1], scales[3 * i + 2]};
         float M[9], Sigma[9], RS[9], Sc[9];
-#pragma unroll
-        for (int a = 0; a < 3; ++a)
-#pragma unroll
-            for (int b = 0; b < 3; ++b) M[a * 3 + b] = Rq[a * 3 + b] * s[b];
-        mat3_mul_bt(M, M, Sigma);
-        mat3_mul(R, Sigma, RS);
-        mat3_mul_bt(RS, R, Sc);
+        world_cov(Rq, s, M, Sigma);
+        cam_cov(R, Sigma, RS, Sc);
 
         const float W = (float)cam.W, H = (float)cam.H;
-        float tanx = 0.5f * W / fx, tany = 0.5f * H / fy;
-        float lxp = (W - cx) / fx + 0.3f * tanx, lxn = cx / fx + 0.3f * tanx;
-        float lyp = (H - cy) / fy + 0.3f * tany, lyn = cy / fy + 0.3f * tany;
-        float rz = 1.0f / z;
-        float rz2 = rz * rz;
-        float xr = x * rz, yr = y * rz;
-        float tx = z * fminf(lxp, fmaxf(-lxn, xr));
-        float ty = z * fminf(lyp, fmaxf(-lyn, yr));
-        float J0 = fx * rz, J2 = -fx * tx * rz2, J4 = fy * rz, J5 = -fy * ty * rz2;
+        const PerspJacobian pj = persp_jacobian(x, y, z, fx, fy, cx, cy, W, H);
+        const float rz = pj.rz, J0 = pj.J[0], J2 = pj.J[2], J4 = pj.J[4], J5 = pj.J[5];
         float k00 = J0 * Sc[0] + J2 * Sc[6], k01 = J0 * Sc[1] + J2 * Sc[7], k02 = J0 * Sc[2] + J2 * Sc[8];
         float k11 = J4 * Sc[4] + J5 * Sc[7], k12 = J4 * Sc[5] + J5 * Sc[8];
         float a = k00 * J0 + k02 * J2;
@@ -204,14 +153,8 @@ project_fwd_kernel(int N, int C, const float* __restrict__ means, const float* _
         float inv = 1.0f / sqrtf(dx * dx + dy * dy + dz * dz);
         float B[16];
         sh_basis(sh_degree, dx * inv, dy * inv, dz * inv, B);
-        const float4* sp = reinterpret_cast<const float4*>(sh + (size_t)i * 48);
         float c48[48];
-#pragma unroll
-        for (int k = 0; k < 12; ++k) {
-            // C > 1: the chunk's other view warps read the same lines next, so let them allocate in L1
-            float4 q = C > 1 ? __ldg(sp + k) : adb_ldg_stream4(sp + k);
-            c48[4 * k] = q.x; c48[4 * k + 1] = q.y; c48[4 * k + 2] = q.z; c48[4 * k + 3] = q.w;
-        }
+        load_sh_coeffs(sh, i, C, c48);          // C > 1: the chunk's C view warps read the same lines
 #pragma unroll
         for (int k = 0; k < 16; ++k) {
             r += B[k] * c48[3 * k]; g += B[k] * c48[3 * k + 1]; bl += B[k] * c48[3 * k + 2];

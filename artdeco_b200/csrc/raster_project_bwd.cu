@@ -4,70 +4,11 @@
 //
 // Replaces gsplat's fully_fused_projection_bwd + spherical_harmonics_bwd reached through autograd of
 // Reconstruct/scene/scene_models/h3dgsv3.py:664-680 (SURVEY.md App. B.6).  Formulas are the analytic
-// backward pinned against torch.autograd in tests/test_oracle_raster.py.
-#include "raster_common.cuh"
+// backward pinned against torch.autograd in tests/test_oracle_raster.py; the projection, covariance and SH pieces
+// shared with the forward and the multi-view backward are in raster_geom.cuh.
+#include "raster_geom.cuh"
 
 namespace {
-
-__device__ __forceinline__ void mat3_mul(const float* A, const float* B, float* C) {
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j)
-            C[i * 3 + j] = A[i * 3 + 0] * B[0 * 3 + j] + A[i * 3 + 1] * B[1 * 3 + j] + A[i * 3 + 2] * B[2 * 3 + j];
-}
-__device__ __forceinline__ void mat3_mul_bt(const float* A, const float* B, float* C) {
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j)
-            C[i * 3 + j] = A[i * 3 + 0] * B[j * 3 + 0] + A[i * 3 + 1] * B[j * 3 + 1] + A[i * 3 + 2] * B[j * 3 + 2];
-}
-__device__ __forceinline__ void mat3_mul_at(const float* A, const float* B, float* C) {
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j)
-            C[i * 3 + j] = A[0 * 3 + i] * B[0 * 3 + j] + A[1 * 3 + i] * B[1 * 3 + j] + A[2 * 3 + i] * B[2 * 3 + j];
-}
-
-// basis and its gradient w.r.t. the unit direction, degree <= 3
-__device__ __forceinline__ void sh_basis_and_grad(int deg, float x, float y, float z, float* B, float* Bx, float* By,
-                                                  float* Bz) {
-#pragma unroll
-    for (int k = 0; k < 16; ++k) B[k] = Bx[k] = By[k] = Bz[k] = 0.f;
-    B[0] = 0.2820947917738781f;
-    if (deg < 1) return;
-    B[1] = -0.48860251190292f * y; B[2] = 0.48860251190292f * z; B[3] = -0.48860251190292f * x;
-    By[1] = -0.48860251190292f; Bz[2] = 0.48860251190292f; Bx[3] = -0.48860251190292f;
-    if (deg < 2) return;
-    const float z2 = z * z, fT0B = -1.092548430592079f * z, fT0B_z = -1.092548430592079f;
-    const float fC1 = x * x - y * y, fS1 = 2.f * x * y;
-    const float fC1_x = 2.f * x, fC1_y = -2.f * y, fS1_x = 2.f * y, fS1_y = 2.f * x;
-    B[4] = 0.5462742152960395f * fS1; B[5] = fT0B * y; B[6] = 0.9461746957575601f * z2 - 0.3153915652525201f;
-    B[7] = fT0B * x; B[8] = 0.5462742152960395f * fC1;
-    Bx[4] = 0.5462742152960395f * fS1_x; By[4] = 0.5462742152960395f * fS1_y;
-    By[5] = fT0B; Bz[5] = fT0B_z * y;
-    Bz[6] = 2.f * 0.9461746957575601f * z;
-    Bx[7] = fT0B; Bz[7] = fT0B_z * x;
-    Bx[8] = 0.5462742152960395f * fC1_x; By[8] = 0.5462742152960395f * fC1_y;
-    if (deg < 3) return;
-    const float fT0C = -2.285228997322329f * z2 + 0.4570457994644658f, fT0C_z = -2.285228997322329f * 2.f * z;
-    const float fT1B = 1.445305721320277f * z, fT1B_z = 1.445305721320277f;
-    const float fC2 = x * fC1 - y * fS1, fS2 = x * fS1 + y * fC1;
-    const float fC2_x = fC1 + x * fC1_x - y * fS1_x, fC2_y = x * fC1_y - fS1 - y * fS1_y;
-    const float fS2_x = fS1 + x * fS1_x + y * fC1_x, fS2_y = x * fS1_y + fC1 + y * fC1_y;
-    B[9] = -0.5900435899266435f * fS2; B[10] = fT1B * fS1; B[11] = fT0C * y;
-    B[12] = z * (1.865881662950577f * z2 - 1.119528997770346f); B[13] = fT0C * x; B[14] = fT1B * fC1;
-    B[15] = -0.5900435899266435f * fC2;
-    Bx[9] = -0.5900435899266435f * fS2_x; By[9] = -0.5900435899266435f * fS2_y;
-    Bx[10] = fT1B * fS1_x; By[10] = fT1B * fS1_y; Bz[10] = fT1B_z * fS1;
-    By[11] = fT0C; Bz[11] = fT0C_z * y;
-    Bz[12] = 3.f * 1.865881662950577f * z2 - 1.119528997770346f;
-    Bx[13] = fT0C; Bz[13] = fT0C_z * x;
-    Bx[14] = fT1B * fC1_x; By[14] = fT1B * fC1_y; Bz[14] = fT1B_z * fC1;
-    Bx[15] = -0.5900435899266435f * fC2_x; By[15] = -0.5900435899266435f * fC2_y;
-}
 
 constexpr int PB = 128;  // threads per block (register heavy kernel)
 
@@ -102,33 +43,12 @@ project_bwd_kernel(int N, const float* __restrict__ means, const float* __restri
         const float4 q4 = reinterpret_cast<const float4*>(quats)[i];
         const float qinv = rsqrtf(q4.x * q4.x + q4.y * q4.y + q4.z * q4.z + q4.w * q4.w);
         const float w = q4.x * qinv, qx = q4.y * qinv, qy = q4.z * qinv, qz = q4.w * qinv;
-        float Rq[9];
-        {
-            float x2 = qx * qx, y2 = qy * qy, z2 = qz * qz;
-            float xy = qx * qy, xz = qx * qz, yz = qy * qz, wx = w * qx, wy = w * qy, wz = w * qz;
-            Rq[0] = 1.0f - 2.0f * (y2 + z2); Rq[1] = 2.0f * (xy - wz);        Rq[2] = 2.0f * (xz + wy);
-            Rq[3] = 2.0f * (xy + wz);        Rq[4] = 1.0f - 2.0f * (x2 + z2); Rq[5] = 2.0f * (yz - wx);
-            Rq[6] = 2.0f * (xz - wy);        Rq[7] = 2.0f * (yz + wx);        Rq[8] = 1.0f - 2.0f * (x2 + y2);
-        }
+        float Rq[9], M[9], Sigma[9], RS[9], Sc[9];
+        quat_to_rotmat(w, qx, qy, qz, Rq);
         const float s[3] = {scales[3 * i], scales[3 * i + 1], scales[3 * i + 2]};
-        float M[9], Sigma[9], RS[9], Sc[9];
-#pragma unroll
-        for (int a = 0; a < 3; ++a)
-#pragma unroll
-            for (int b = 0; b < 3; ++b) M[a * 3 + b] = Rq[a * 3 + b] * s[b];
-        mat3_mul_bt(M, M, Sigma);
-        mat3_mul(R, Sigma, RS);
-        mat3_mul_bt(RS, R, Sc);
-
-        const float Wf = (float)cam.W, Hf = (float)cam.H;
-        const float tanx = 0.5f * Wf / fx, tany = 0.5f * Hf / fy;
-        const float lxp = (Wf - cx) / fx + 0.3f * tanx, lxn = cx / fx + 0.3f * tanx;
-        const float lyp = (Hf - cy) / fy + 0.3f * tany, lyn = cy / fy + 0.3f * tany;
-        const float rz = 1.0f / z, rz2 = rz * rz, rz3 = rz2 * rz;
-        const float xr = x * rz, yr = y * rz;
-        const bool clamp_x = !(xr <= lxp && xr >= -lxn), clamp_y = !(yr <= lyp && yr >= -lyn);
-        const float tx = z * fminf(lxp, fmaxf(-lxn, xr)), ty = z * fminf(lyp, fmaxf(-lyn, yr));
-        const float J[6] = {fx * rz, 0.f, -fx * tx * rz2, 0.f, fy * rz, -fy * ty * rz2};
+        world_cov(Rq, s, M, Sigma);
+        cam_cov(R, Sigma, RS, Sc);
+        const PerspJacobian pj = persp_jacobian(x, y, z, fx, fy, cx, cy, (float)cam.W, (float)cam.H);
 
         const float4 rec0 = reinterpret_cast<const float4*>(splats + (size_t)i * ADB_SPLAT_STRIDE)[0];
         const float4 rec1 = reinterpret_cast<const float4*>(splats + (size_t)i * ADB_SPLAT_STRIDE)[1];
@@ -136,6 +56,9 @@ project_bwd_kernel(int N, const float* __restrict__ means, const float* __restri
         const float4 g0 = reinterpret_cast<const float4*>(v_splats + (size_t)i * ADB_SPLAT_STRIDE)[0];
         const float4 g1 = reinterpret_cast<const float4*>(v_splats + (size_t)i * ADB_SPLAT_STRIDE)[1];
         const float4 g2 = reinterpret_cast<const float4*>(v_splats + (size_t)i * ADB_SPLAT_STRIDE)[2];
+        const float* J = pj.J;
+        const float rz = pj.rz, rz2 = pj.rz2, rz3 = pj.rz3, tx = pj.tx, ty = pj.ty;
+        const bool clamp_x = pj.clamp_x, clamp_y = pj.clamp_y;
         const float A = rec0.z, B = rec0.w, C = rec1.x;
         // blend_bwd accumulates raw moments of v_sigma about the splat centre (slots 0..5 = M1x M1y M2xx M2xy M2yy M0):
         //   v_mean2d = conic * (M1x, M1y);  v_conic = (M2xx/2, M2xy, M2yy/2);  v_opacity = -M0 / opacity
@@ -171,9 +94,9 @@ project_bwd_kernel(int N, const float* __restrict__ means, const float* __restri
         vp[2] = -(fx * x * vu + fy * y * vv) * rz2 + v_depth;
         vp[2] += -fx * rz2 * vJ[0] - fy * rz2 * vJ[4];
         if (!clamp_x) { vp[0] += -fx * rz2 * vJ[2]; vp[2] += 2.0f * fx * tx * rz3 * vJ[2]; }
-        else          { vp[2] += fx * tx * rz3 * vJ[2]; }
+        else             { vp[2] += fx * tx * rz3 * vJ[2]; }
         if (!clamp_y) { vp[1] += -fy * rz2 * vJ[5]; vp[2] += 2.0f * fy * ty * rz3 * vJ[5]; }
-        else          { vp[2] += fy * ty * rz3 * vJ[5]; }
+        else             { vp[2] += fy * ty * rz3 * vJ[5]; }
 #pragma unroll
         for (int a = 0; a < 3; ++a) {
             vm[a] = R[0 * 3 + a] * vp[0] + R[1 * 3 + a] * vp[1] + R[2 * 3 + a] * vp[2];
@@ -181,32 +104,13 @@ project_bwd_kernel(int N, const float* __restrict__ means, const float* __restri
 #pragma unroll
             for (int b = 0; b < 3; ++b) red[a * 3 + b] = vp[a] * mu[b];
         }
-        float tmp[9], vSigma[9], RSig[9], add[9];
+        float tmp[9], vSigma[9], add[9];
         mat3_mul_at(R, vSc, tmp);
         mat3_mul(tmp, R, vSigma);
-        mat3_mul(R, Sigma, RSig);
-        mat3_mul(vSc, RSig, add);
+        mat3_mul(vSc, RS, add);
 #pragma unroll
         for (int k = 0; k < 9; ++k) red[k] += 2.0f * add[k];
-        float vM[9], vRq[9];
-        mat3_mul(vSigma, M, vM);
-#pragma unroll
-        for (int a = 0; a < 3; ++a)
-#pragma unroll
-            for (int b = 0; b < 3; ++b) {
-                vM[a * 3 + b] *= 2.0f;
-                vRq[a * 3 + b] = vM[a * 3 + b] * s[b];
-            }
-#pragma unroll
-        for (int b = 0; b < 3; ++b) vs[b] = vM[b] * Rq[b] + vM[3 + b] * Rq[3 + b] + vM[6 + b] * Rq[6 + b];
-        float vn[4];
-        vn[0] = 2.0f * (qx * (vRq[7] - vRq[5]) + qy * (vRq[2] - vRq[6]) + qz * (vRq[3] - vRq[1]));
-        vn[1] = 2.0f * (-2.0f * qx * (vRq[4] + vRq[8]) + qy * (vRq[1] + vRq[3]) + qz * (vRq[2] + vRq[6]) + w * (vRq[7] - vRq[5]));
-        vn[2] = 2.0f * (qx * (vRq[1] + vRq[3]) - 2.0f * qy * (vRq[0] + vRq[8]) + qz * (vRq[5] + vRq[7]) + w * (vRq[2] - vRq[6]));
-        vn[3] = 2.0f * (qx * (vRq[2] + vRq[6]) + qy * (vRq[5] + vRq[7]) - 2.0f * qz * (vRq[0] + vRq[4]) + w * (vRq[3] - vRq[1]));
-        const float dotq = vn[0] * w + vn[1] * qx + vn[2] * qy + vn[3] * qz;
-        vq[0] = (vn[0] - dotq * w) * qinv; vq[1] = (vn[1] - dotq * qx) * qinv;
-        vq[2] = (vn[2] - dotq * qy) * qinv; vq[3] = (vn[3] - dotq * qz) * qinv;
+        world_cov_bwd(vSigma, M, Rq, s, w, qx, qy, qz, qinv, vs, vq);
 
         // SH backward (+ its contribution to v_means / v_campos)
         if (sh) {
@@ -214,20 +118,15 @@ project_bwd_kernel(int N, const float* __restrict__ means, const float* __restri
             const float inv = rsqrtf(dx * dx + dy * dy + dz * dz);
             const float nx = dx * inv, ny = dy * inv, nz = dz * inv;
             float Bs[16], Bx[16], By[16], Bz[16];
-            sh_basis_and_grad(sh_degree, nx, ny, nz, Bs, Bx, By, Bz);
+            sh_basis_grad(sh_degree, nx, ny, nz, Bs, Bx, By, Bz);
             const float rgb[3] = {rec2.x, rec2.y, rec2.z};
             float gch[3];
 #pragma unroll
             for (int c = 0; c < 3; ++c) gch[c] = rgb[c] > 0.f ? v_rgb[c] : 0.f;
-            const float4* sp = reinterpret_cast<const float4*>(sh + (size_t)i * 48);
             float4* op = reinterpret_cast<float4*>(v_sh + (size_t)i * 48);
             float vnx = 0.f, vny = 0.f, vnz = 0.f;
             float c48[48];
-#pragma unroll
-            for (int k = 0; k < 12; ++k) {
-                float4 q = adb_ldg_stream4(sp + k);
-                c48[4 * k] = q.x; c48[4 * k + 1] = q.y; c48[4 * k + 2] = q.z; c48[4 * k + 3] = q.w;
-            }
+            load_sh_coeffs(sh, i, 1, c48);
             float o48[48];
 #pragma unroll
             for (int k = 0; k < 16; ++k)

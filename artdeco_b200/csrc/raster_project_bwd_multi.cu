@@ -11,33 +11,12 @@
 //                      direction term is added to v_means.
 // The split is also what makes the multi-GPU exchange cheap (artdeco_b200/parallel.py): ranks all-gather g_rgb (12 B per view
 // and Gaussian) and all-reduce only the 11 geometry floats instead of all-reducing 59 floats; every rank then expands the SH
-// gradient of ALL views locally.  Formulas: raster_project_bwd.cu (SURVEY.md App. B.6), pinned by tests against the sum of
-// single-view backward passes.
-#include "raster_common.cuh"
+// gradient of ALL views locally.  The shared projection and SH math is in raster_geom.cuh (SURVEY.md App. B.6); the per-view
+// backward chain and its clamped Jacobian are written out here as in raster_project_bwd.cu, because sharing them changes the
+// compiled kernels.  Pinned by tests against the sum of single-view backward passes.
+#include "raster_geom.cuh"
 
 namespace {
-
-__device__ __forceinline__ void m3_mul(const float* A, const float* B, float* C) {
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j)
-            C[i * 3 + j] = A[i * 3 + 0] * B[0 * 3 + j] + A[i * 3 + 1] * B[1 * 3 + j] + A[i * 3 + 2] * B[2 * 3 + j];
-}
-__device__ __forceinline__ void m3_mul_bt(const float* A, const float* B, float* C) {
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j)
-            C[i * 3 + j] = A[i * 3 + 0] * B[j * 3 + 0] + A[i * 3 + 1] * B[j * 3 + 1] + A[i * 3 + 2] * B[j * 3 + 2];
-}
-__device__ __forceinline__ void m3_mul_at(const float* A, const float* B, float* C) {
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j)
-            C[i * 3 + j] = A[0 * 3 + i] * B[0 * 3 + j] + A[1 * 3 + i] * B[1 * 3 + j] + A[2 * 3 + i] * B[2 * 3 + j];
-}
 
 constexpr int PB = 128;
 
@@ -61,18 +40,8 @@ project_bwd_multi_kernel(int N, int C, const float* __restrict__ means, const fl
         s[0] = scales[3 * i]; s[1] = scales[3 * i + 1]; s[2] = scales[3 * i + 2];
     }
     float Rq[9], M[9], Sigma[9];
-    {
-        const float x2 = qx * qx, y2 = qy * qy, z2 = qz * qz;
-        const float xy = qx * qy, xz = qx * qz, yz = qy * qz, wx = w * qx, wy = w * qy, wz = w * qz;
-        Rq[0] = 1.0f - 2.0f * (y2 + z2); Rq[1] = 2.0f * (xy - wz);        Rq[2] = 2.0f * (xz + wy);
-        Rq[3] = 2.0f * (xy + wz);        Rq[4] = 1.0f - 2.0f * (x2 + z2); Rq[5] = 2.0f * (yz - wx);
-        Rq[6] = 2.0f * (xz - wy);        Rq[7] = 2.0f * (yz + wx);        Rq[8] = 1.0f - 2.0f * (x2 + y2);
-#pragma unroll
-        for (int a = 0; a < 3; ++a)
-#pragma unroll
-            for (int b = 0; b < 3; ++b) M[a * 3 + b] = Rq[a * 3 + b] * s[b];
-        m3_mul_bt(M, M, Sigma);
-    }
+    quat_to_rotmat(w, qx, qy, qz, Rq);
+    world_cov(Rq, s, M, Sigma);
     float vm[3] = {0.f, 0.f, 0.f}, vo = 0.f;
     float vSigma_acc[9];
 #pragma unroll
@@ -98,8 +67,7 @@ project_bwd_multi_kernel(int N, int C, const float* __restrict__ means, const fl
             const float y = R[3] * mu[0] + R[4] * mu[1] + R[5] * mu[2] + t[1];
             const float z = R[6] * mu[0] + R[7] * mu[1] + R[8] * mu[2] + t[2];
             float RS[9], Sc[9];
-            m3_mul(R, Sigma, RS);
-            m3_mul_bt(RS, R, Sc);
+            cam_cov(R, Sigma, RS, Sc);
             const float Wf = (float)W, Hf = (float)H;
             const float tanx = 0.5f * Wf / fx, tany = 0.5f * Hf / fy;
             const float lxp = (Wf - cx) / fx + 0.3f * tanx, lxn = cx / fx + 0.3f * tanx;
@@ -161,9 +129,9 @@ project_bwd_multi_kernel(int N, int C, const float* __restrict__ means, const fl
                 for (int b = 0; b < 3; ++b) red[a * 3 + b] = vp[a] * mu[b];
             }
             float tmp[9], vSigma[9], add[9];
-            m3_mul_at(R, vSc, tmp);
-            m3_mul(tmp, R, vSigma);
-            m3_mul(vSc, RS, add);
+            mat3_mul_at(R, vSc, tmp);
+            mat3_mul(tmp, R, vSigma);
+            mat3_mul(vSc, RS, add);
 #pragma unroll
             for (int k = 0; k < 9; ++k) { red[k] += 2.0f * add[k]; vSigma_acc[k] += vSigma[k]; }
         }
@@ -194,66 +162,12 @@ project_bwd_multi_kernel(int N, int C, const float* __restrict__ means, const fl
     }
     if (!in) return;
     // Sigma = M M^T chain, once for the summed v_Sigma (linear in v_Sigma)
-    float vM[9], vRq[9], vs[3], vq[4];
-    m3_mul(vSigma_acc, M, vM);
-#pragma unroll
-    for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int b = 0; b < 3; ++b) {
-            vM[a * 3 + b] *= 2.0f;
-            vRq[a * 3 + b] = vM[a * 3 + b] * s[b];
-        }
-#pragma unroll
-    for (int b = 0; b < 3; ++b) vs[b] = vM[b] * Rq[b] + vM[3 + b] * Rq[3 + b] + vM[6 + b] * Rq[6 + b];
-    float vn[4];
-    vn[0] = 2.0f * (qx * (vRq[7] - vRq[5]) + qy * (vRq[2] - vRq[6]) + qz * (vRq[3] - vRq[1]));
-    vn[1] = 2.0f * (-2.0f * qx * (vRq[4] + vRq[8]) + qy * (vRq[1] + vRq[3]) + qz * (vRq[2] + vRq[6]) + w * (vRq[7] - vRq[5]));
-    vn[2] = 2.0f * (qx * (vRq[1] + vRq[3]) - 2.0f * qy * (vRq[0] + vRq[8]) + qz * (vRq[5] + vRq[7]) + w * (vRq[2] - vRq[6]));
-    vn[3] = 2.0f * (qx * (vRq[2] + vRq[6]) + qy * (vRq[5] + vRq[7]) - 2.0f * qz * (vRq[0] + vRq[4]) + w * (vRq[3] - vRq[1]));
-    const float dotq = vn[0] * w + vn[1] * qx + vn[2] * qy + vn[3] * qz;
-    vq[0] = (vn[0] - dotq * w) * qinv; vq[1] = (vn[1] - dotq * qx) * qinv;
-    vq[2] = (vn[2] - dotq * qy) * qinv; vq[3] = (vn[3] - dotq * qz) * qinv;
+    float vs[3], vq[4];
+    world_cov_bwd(vSigma_acc, M, Rq, s, w, qx, qy, qz, qinv, vs, vq);
     v_means[3 * i] = vm[0]; v_means[3 * i + 1] = vm[1]; v_means[3 * i + 2] = vm[2];
     reinterpret_cast<float4*>(v_quats)[i] = make_float4(vq[0], vq[1], vq[2], vq[3]);
     v_scales[3 * i] = vs[0]; v_scales[3 * i + 1] = vs[1]; v_scales[3 * i + 2] = vs[2];
     v_opac[i] = vo;
-}
-
-// basis and its gradient w.r.t. the unit direction, degree <= 3 (same polynomials as raster_project_bwd.cu)
-__device__ __forceinline__ void sh_basis_grad(int deg, float x, float y, float z, float* B, float* Bx, float* By, float* Bz) {
-#pragma unroll
-    for (int k = 0; k < 16; ++k) B[k] = Bx[k] = By[k] = Bz[k] = 0.f;
-    B[0] = 0.2820947917738781f;
-    if (deg < 1) return;
-    B[1] = -0.48860251190292f * y; B[2] = 0.48860251190292f * z; B[3] = -0.48860251190292f * x;
-    By[1] = -0.48860251190292f; Bz[2] = 0.48860251190292f; Bx[3] = -0.48860251190292f;
-    if (deg < 2) return;
-    const float z2 = z * z, fT0B = -1.092548430592079f * z, fT0B_z = -1.092548430592079f;
-    const float fC1 = x * x - y * y, fS1 = 2.f * x * y;
-    const float fC1_x = 2.f * x, fC1_y = -2.f * y, fS1_x = 2.f * y, fS1_y = 2.f * x;
-    B[4] = 0.5462742152960395f * fS1; B[5] = fT0B * y; B[6] = 0.9461746957575601f * z2 - 0.3153915652525201f;
-    B[7] = fT0B * x; B[8] = 0.5462742152960395f * fC1;
-    Bx[4] = 0.5462742152960395f * fS1_x; By[4] = 0.5462742152960395f * fS1_y;
-    By[5] = fT0B; Bz[5] = fT0B_z * y;
-    Bz[6] = 2.f * 0.9461746957575601f * z;
-    Bx[7] = fT0B; Bz[7] = fT0B_z * x;
-    Bx[8] = 0.5462742152960395f * fC1_x; By[8] = 0.5462742152960395f * fC1_y;
-    if (deg < 3) return;
-    const float fT0C = -2.285228997322329f * z2 + 0.4570457994644658f, fT0C_z = -2.285228997322329f * 2.f * z;
-    const float fT1B = 1.445305721320277f * z, fT1B_z = 1.445305721320277f;
-    const float fC2 = x * fC1 - y * fS1, fS2 = x * fS1 + y * fC1;
-    const float fC2_x = fC1 + x * fC1_x - y * fS1_x, fC2_y = x * fC1_y - fS1 - y * fS1_y;
-    const float fS2_x = fS1 + x * fS1_x + y * fC1_x, fS2_y = x * fS1_y + fC1 + y * fC1_y;
-    B[9] = -0.5900435899266435f * fS2; B[10] = fT1B * fS1; B[11] = fT0C * y;
-    B[12] = z * (1.865881662950577f * z2 - 1.119528997770346f); B[13] = fT0C * x; B[14] = fT1B * fC1;
-    B[15] = -0.5900435899266435f * fC2;
-    Bx[9] = -0.5900435899266435f * fS2_x; By[9] = -0.5900435899266435f * fS2_y;
-    Bx[10] = fT1B * fS1_x; By[10] = fT1B * fS1_y; Bz[10] = fT1B_z * fS1;
-    By[11] = fT0C; Bz[11] = fT0C_z * y;
-    Bz[12] = 3.f * 1.865881662950577f * z2 - 1.119528997770346f;
-    Bx[13] = fT0C; Bz[13] = fT0C_z * x;
-    Bx[14] = fT1B * fC1_x; By[14] = fT1B * fC1_y; Bz[14] = fT1B_z * fC1;
-    Bx[15] = -0.5900435899266435f * fC2_x; By[15] = -0.5900435899266435f * fC2_y;
 }
 
 __global__ void __launch_bounds__(PB)
@@ -353,26 +267,6 @@ sh_bwd_multi_kernel(int N, int C, const float* __restrict__ means, const float* 
 // replicated part — the expansion of ALL views on every rank — without the 192 B coefficient read, the basis gradients and
 // half of the registers.
 
-// basis values only, degree <= 3
-__device__ __forceinline__ void sh_basis_values(int deg, float x, float y, float z, float* B) {
-#pragma unroll
-    for (int k = 1; k < 16; ++k) B[k] = 0.f;
-    B[0] = 0.2820947917738781f;
-    if (deg < 1) return;
-    B[1] = -0.48860251190292f * y; B[2] = 0.48860251190292f * z; B[3] = -0.48860251190292f * x;
-    if (deg < 2) return;
-    const float z2 = z * z, fT0B = -1.092548430592079f * z;
-    const float fC1 = x * x - y * y, fS1 = 2.f * x * y;
-    B[4] = 0.5462742152960395f * fS1; B[5] = fT0B * y; B[6] = 0.9461746957575601f * z2 - 0.3153915652525201f;
-    B[7] = fT0B * x; B[8] = 0.5462742152960395f * fC1;
-    if (deg < 3) return;
-    const float fT0C = -2.285228997322329f * z2 + 0.4570457994644658f, fT1B = 1.445305721320277f * z;
-    const float fC2 = x * fC1 - y * fS1, fS2 = x * fS1 + y * fC1;
-    B[9] = -0.5900435899266435f * fS2; B[10] = fT1B * fS1; B[11] = fT0C * y;
-    B[12] = z * (1.865881662950577f * z2 - 1.119528997770346f); B[13] = fT0C * x; B[14] = fT1B * fC1;
-    B[15] = -0.5900435899266435f * fC2;
-}
-
 // v_sh[i] = sum_c basis(dir_c(i)) (x) g_rgb[c][i]   (overwritten)
 __global__ void __launch_bounds__(PB)
 sh_expand_multi_kernel(int N, int C, const float* __restrict__ means, int sh_degree, const float* __restrict__ campos,
@@ -395,7 +289,7 @@ sh_expand_multi_kernel(int N, int C, const float* __restrict__ means, int sh_deg
         const float dx = mx - campos[3 * c], dy = my - campos[3 * c + 1], dz = mz - campos[3 * c + 2];
         const float inv = rsqrtf(dx * dx + dy * dy + dz * dz);
         float Bs[16];
-        sh_basis_values(sh_degree, dx * inv, dy * inv, dz * inv, Bs);
+        sh_basis(sh_degree, dx * inv, dy * inv, dz * inv, Bs);
 #pragma unroll
         for (int k = 0; k < 16; ++k) {
             o48[3 * k] = fmaf(Bs[k], g0, o48[3 * k]);

@@ -20,7 +20,7 @@ from typing import NamedTuple
 import torch
 
 from . import _lib
-from .raster import _f32c, blend_backward, blend_forward, intersect, project
+from .raster import _f32c, blend_backward, blend_forward, intersect, project, project_backward
 
 EPS2D_INRIA = 0.3
 NEAR_INRIA = 0.2
@@ -77,18 +77,9 @@ class _RasterizeLegacy(torch.autograd.Function):
             gx = torch.where(live, ca * v_splats[:, 0] + cb * v_splats[:, 1], torch.zeros_like(ca))
             gy = torch.where(live, cb * v_splats[:, 0] + cc * v_splats[:, 1], torch.zeros_like(ca))
             v_means2D = torch.stack([gx * (0.5 * W), gy * (0.5 * H), torch.zeros_like(gx)], -1)
-            v_means = torch.empty_like(means)
-            v_quats = torch.empty_like(quats)
-            v_scales = torch.empty_like(scales)
-            v_opac = torch.empty_like(opacities)
-            v_sh = torch.empty_like(sh)
-            v_view = torch.zeros(4, 4, dtype=torch.float32, device=dev)
-            v_campos = torch.zeros(3, dtype=torch.float32, device=dev)
-            _lib.call("adb_raster_project_bwd", N, _lib.ptr(means), _lib.ptr(quats), _lib.ptr(scales), _lib.ptr(sh),
-                      int(sh_degree), _lib.ptr(viewmat), _lib.ptr(K), _lib.ptr(campos), W, H, EPS2D_INRIA, NEAR_INRIA,
-                      1e10, 0.0, _lib.ptr(radii), _lib.ptr(splats), _lib.ptr(v_splats), _lib.ptr(v_means),
-                      _lib.ptr(v_quats), _lib.ptr(v_scales), _lib.ptr(v_opac), _lib.ptr(v_sh), _lib.ptr(v_view),
-                      _lib.ptr(v_campos), _lib.stream())
+            v_means, v_quats, v_scales, v_opac, v_sh, v_view, v_campos = project_backward(
+                means, quats, scales, opacities, sh, sh_degree, viewmat, K, campos, W, H, EPS2D_INRIA, NEAR_INRIA, 1e10, 0.0,
+                radii, splats, v_splats)
         return (v_means, v_means2D, v_quats, v_scales, v_opac, v_sh, v_view, None, v_campos, None, None, None)
 
 

@@ -111,6 +111,26 @@ def project(means, quats, scales, opacities, sh, sh_degree, viewmat, K, campos, 
     return radii, splats, tpg
 
 
+def project_backward(means, quats, scales, opacities, sh, sh_degree, viewmat, K, campos, W, H, eps2d, near, far,
+                     radius_clip, radii, splats, v_splats):
+    """Projection + SH backward of one camera (``project``'s arguments, its radii / splats, and the blend backward's
+    ``v_splats``).  Returns (v_means, v_quats, v_scales, v_opac, v_sh, v_viewmat[4,4], v_campos[3]); with ``sh=None``
+    v_sh and v_campos are None."""
+    dev = means.device
+    v_means = torch.empty_like(means)
+    v_quats = torch.empty_like(quats)
+    v_scales = torch.empty_like(scales)
+    v_opac = torch.empty_like(opacities)
+    v_sh = torch.empty_like(sh) if sh is not None else None
+    v_view = torch.zeros(4, 4, dtype=torch.float32, device=dev)
+    v_campos = torch.zeros(3, dtype=torch.float32, device=dev) if sh is not None else None
+    _lib.call("adb_raster_project_bwd", means.shape[0], _lib.ptr(means), _lib.ptr(quats), _lib.ptr(scales), _lib.ptr(sh),
+              int(sh_degree), _lib.ptr(viewmat), _lib.ptr(K), _lib.ptr(campos), W, H, eps2d, near, far, radius_clip,
+              _lib.ptr(radii), _lib.ptr(splats), _lib.ptr(v_splats), _lib.ptr(v_means), _lib.ptr(v_quats),
+              _lib.ptr(v_scales), _lib.ptr(v_opac), _lib.ptr(v_sh), _lib.ptr(v_view), _lib.ptr(v_campos), _lib.stream())
+    return v_means, v_quats, v_scales, v_opac, v_sh, v_view, v_campos
+
+
 def new_tile_counts(W, H, dev, views=None):
     """Zeroed counter buffer of the tile-bucketed intersection: 4 replicated counters per tile, then their segment starts.
     ``views``: C -> one such block per view, [C, 2*4*T] (``project_multi`` / ``intersect_multi``)."""
@@ -388,18 +408,9 @@ class _RasterizeOneCamera(torch.autograd.Function):
         v_alphas = torch.zeros(H, W, device=dev) if v_alphas is None else _f32c(v_alphas)
         with torch.cuda.device(dev):
             v_splats = blend_backward(W, H, N, splats, vals, offsets, alphas, last_ids, v_colors, v_alphas, hits=ctx.hits)
-            v_means = torch.empty_like(means)
-            v_quats = torch.empty_like(quats)
-            v_scales = torch.empty_like(scales)
-            v_opac = torch.empty_like(opacities)
-            v_sh = torch.empty_like(sh) if sh is not None else None
-            v_view = torch.zeros(4, 4, dtype=torch.float32, device=dev)
-            v_campos = torch.zeros(3, dtype=torch.float32, device=dev) if sh is not None else None
-            _lib.call("adb_raster_project_bwd", N, _lib.ptr(means), _lib.ptr(quats), _lib.ptr(scales), _lib.ptr(sh),
-                      int(sh_degree), _lib.ptr(viewmat), _lib.ptr(K), _lib.ptr(campos), W, H, eps2d, near, far,
-                      radius_clip, _lib.ptr(radii), _lib.ptr(splats), _lib.ptr(v_splats), _lib.ptr(v_means),
-                      _lib.ptr(v_quats), _lib.ptr(v_scales), _lib.ptr(v_opac), _lib.ptr(v_sh), _lib.ptr(v_view),
-                      _lib.ptr(v_campos), _lib.stream())
+            v_means, v_quats, v_scales, v_opac, v_sh, v_view, v_campos = project_backward(
+                means, quats, scales, opacities, sh, sh_degree, viewmat, K, campos, W, H, eps2d, near, far, radius_clip,
+                radii, splats, v_splats)
         v_direct = None
         if direct:
             live = (radii > 0).any(-1, keepdim=True)
