@@ -151,6 +151,47 @@ __device__ __forceinline__ void load_sh_coeffs(const float* sh, int i, int reade
     }
 }
 
+// ---- staging a CTA's parameter rows in shared memory -------------------------------------------------------------------
+// One lane per Gaussian reading its own 192 B SH row makes every 16 B load instruction touch 32 different 128 B lines; copying
+// a CTA's contiguous rows with consecutive threads on consecutive 16 B pieces touches each line once.  Staged SH rows are
+// SH_ROW floats apart: 13 16-byte bank groups, odd, so 8 consecutive lanes' 16 B accesses to the same offset of their own rows
+// fall in 8 distinct groups (48 floats would be a 16-way conflict).
+constexpr int SH_ROW = 52;
+
+// Asynchronous global -> shared copies (cp.async): 16 B bypassing L1, 4 B through it.  cp_async_wait_all waits for the
+// calling thread's copies; a barrier then makes every thread's copies visible to the CTA.
+__device__ __forceinline__ void cp_async16(void* s, const void* g) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(s)), "l"(g) : "memory");
+}
+__device__ __forceinline__ void cp_async4(void* s, const void* g) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((unsigned)__cvta_generic_to_shared(s)), "l"(g) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+// Rows [first, first + n) of a [*, 48] table into shared rows of SH_ROW floats, by all threads of the CTA (asynchronous: the
+// caller waits and synchronises).
+__device__ __forceinline__ void stage_sh_rows(float* s, const float* g, int first, int n) {
+    const float4* src = reinterpret_cast<const float4*>(g + (size_t)first * 48);
+    for (int j = threadIdx.x; j < 12 * n; j += blockDim.x) {
+        const int r = j / 12;
+        cp_async16(s + r * SH_ROW + 4 * (j - 12 * r), src + j);
+    }
+}
+
+// The reverse, after a barrier: shared rows of SH_ROW floats -> rows [first, first + n) of a [*, 48] table.
+__device__ __forceinline__ void store_sh_rows(float* g, const float* s, int first, int n) {
+    float4* dst = reinterpret_cast<float4*>(g + (size_t)first * 48);
+    for (int j = threadIdx.x; j < 12 * n; j += blockDim.x) {
+        const int r = j / 12;
+        dst[j] = *reinterpret_cast<const float4*>(s + r * SH_ROW + 4 * (j - 12 * r));
+    }
+}
+
+// n consecutive floats (4 B copies, for rows of 1 or 3 floats whose start need not be 16 B aligned).
+__device__ __forceinline__ void stage_floats(float* s, const float* g, int n) {
+    for (int j = threadIdx.x; j < n; j += blockDim.x) cp_async4(s + j, g + j);
+}
+
 // dL/dSigma -> dL/d(scales) and dL/d(quats) through Sigma = M M^T, M = Rq diag(s) (world_cov) and the normalisation of
 // q = (w, qx, qy, qz) / qinv.
 __device__ __forceinline__ void world_cov_bwd(const float* vSigma, const float* M, const float* Rq, const float* s, float w,

@@ -15,26 +15,56 @@ namespace {
 
 // C cameras (viewmat / K / campos point at [C,16] / [C,9] / [C,3]); outputs are [C,N,...] stacks and tile_counts holds C
 // consecutive counter blocks of 2 * COPIES * T.  Work split: warp w of the grid handles view (w % C) of the 32 Gaussians of
-// chunk (w / C).  The C warps of a chunk are consecutive, so they run close together (in one CTA when C divides 8, as for
-// the 8-view batch; otherwise a chunk may straddle two neighbouring CTAs) and DRAM delivers the chunk's parameters and SH
-// coefficients once while the other warps hit L1 / L2; the C per-view chains run in parallel.  Each view warp recomputes the
-// quaternion rotation and world-space covariance (a few dozen FP32 ops, against a chain of several hundred per view).  One
-// thread looping over the views, with that work and the SH coefficients kept in registers, needed 110 registers (2 CTAs per
-// SM) and measured 1.48 ms per 8-view batch at 1M Gaussians / 1080p on an H100 SXM at 400 W — no faster than 8 single-view
-// launches (1.42 ms); this split measured 0.78 ms.  For C = 1 it is the single-view kernel thread for thread.  Everything per
-// view is expression for expression the single-view arithmetic, so C = 1 and C > 1 produce the same bits.
+// chunk (w / C).  The C warps of a chunk are consecutive, so the C per-view chains run in parallel.  Each view warp recomputes
+// the quaternion rotation and world-space covariance (a few dozen FP32 ops, against a chain of several hundred per view).
+// One thread looping over the views, with that work and the SH coefficients kept in registers, needed 110 registers (2 CTAs
+// per SM) and measured 1.48 ms per 8-view batch at 1M Gaussians / 1080p on an H100 SXM at 400 W — no faster than 8
+// single-view launches (1.42 ms); this split measured 0.78 ms with every lane loading its own rows from global memory.
+// For C = 1 it is the single-view kernel thread for thread.  Everything per view is expression for expression the
+// single-view arithmetic, so C = 1 and C > 1 produce the same bits.
+//
+// When C divides 8 (the 8-view batch, the single view) or is a multiple of 8, a CTA's warps cover whole chunks, proj_rows(C)
+// consecutive Gaussians; the CTA first copies their parameter rows into shared memory with coalesced copies (raster_geom.cuh:
+// the per-lane 192 B SH rows touched 32 lines per load instruction, and every view warp repeated that), and each view warp
+// reads its lane's row from there.  On an H100 SXM at 700 W this took the 8-view batch from 0.785 to 0.600 ms and the single
+// view from 0.175 to 0.141 ms.  For any other C a chunk straddles two CTAs and the lanes read global memory directly.
 constexpr int PROJ_WARPS = 8;
+constexpr int PROJ_ROW_FLOATS = SH_ROW + 4 + 3 + 3 + 1;        // staged row: SH, quat, mean, scale, opacity
+__host__ __device__ constexpr int proj_rows(int C) {
+    return (C <= PROJ_WARPS && PROJ_WARPS % C == 0) ? PROJ_WARPS * 32 / C : (C % PROJ_WARPS == 0 ? 32 : 0);
+}
 __global__ void __launch_bounds__(PROJ_WARPS * 32)
 project_fwd_kernel(int N, int C, const float* __restrict__ means, const float* __restrict__ quats,
                    const float* __restrict__ scales, const float* __restrict__ opacities,
                    const float* __restrict__ sh, int sh_degree, AdbCam cam,
                    int32_t* __restrict__ radii, float* __restrict__ splats, int32_t* __restrict__ tiles_per_gauss,
                    int32_t* __restrict__ tile_counts) {
+    extern __shared__ float4 proj_smem[];
     const unsigned gw = blockIdx.x * PROJ_WARPS + (threadIdx.x >> 5);     // < 2^32: checked at launch
     const int c = C == 1 ? 0 : (int)(gw % (unsigned)C);                     // C = 1: no integer division
     const unsigned chunk = C == 1 ? gw : gw / (unsigned)C;
     const int i = (int)(chunk * 32u + (threadIdx.x & 31));                 // < N + 32 <= 2^31 - 1: checked at launch
+    // staged rows [first, first + rows): SH rows of SH_ROW floats, then quats, means, scales, opacities
+    const int rows = proj_rows(C);
+    const int first = (int)((blockIdx.x * PROJ_WARPS) / (unsigned)C * 32u);
+    float* const sSH = reinterpret_cast<float*>(proj_smem);
+    float4* const sQ = proj_smem + rows * (SH_ROW / 4);
+    float* const sM = reinterpret_cast<float*>(sQ + rows);
+    float* const sS = sM + 3 * rows;
+    float* const sO = sS + 3 * rows;
+    if (rows) {
+        const int n = min(rows, N - first);                 // > 0: the CTA's first warp has Gaussians
+        if (sh) stage_sh_rows(sSH, sh, first, n);
+        const float4* q4 = reinterpret_cast<const float4*>(quats) + first;
+        for (int j = threadIdx.x; j < n; j += blockDim.x) cp_async16(sQ + j, q4 + j);
+        stage_floats(sM, means + 3 * (size_t)first, 3 * n);
+        stage_floats(sS, scales + 3 * (size_t)first, 3 * n);
+        stage_floats(sO, opacities + first, n);
+        cp_async_wait_all();
+        __syncthreads();
+    }
     if (i >= N) return;
+    const int row = i - first;                             // staged row of Gaussian i
     const size_t ci = (size_t)c * N + i;
     int tr_x0 = 0, tr_x1 = 0, tr_y0 = 0, tr_y1 = 0;    // tile rectangle (for the fused per-tile counting)
     const float* V = cam.viewmat + 16 * c;
@@ -42,23 +72,25 @@ project_fwd_kernel(int N, int C, const float* __restrict__ means, const float* _
     const float R[9] = {V[0], V[1], V[2], V[4], V[5], V[6], V[8], V[9], V[10]};
     const float t[3] = {V[3], V[7], V[11]};
     const float fx = Kc[0], fy = Kc[4], cx = Kc[2], cy = Kc[5];
-    const float m0 = means[3 * i], m1 = means[3 * i + 1], m2 = means[3 * i + 2];
+    const float m0 = rows ? sM[3 * row] : means[3 * i], m1 = rows ? sM[3 * row + 1] : means[3 * i + 1],
+                m2 = rows ? sM[3 * row + 2] : means[3 * i + 2];
 
     int rx_i = 0, ry_i = 0, count = 0, cull_rx = 0, cull_ry = 0;
     float u = 0.f, v = 0.f, ca = 0.f, cb = 0.f, cc = 0.f, lg = 0.f;
     const float x = R[0] * m0 + R[1] * m1 + R[2] * m2 + t[0];
     const float y = R[3] * m0 + R[4] * m1 + R[5] * m2 + t[1];
     const float z = R[6] * m0 + R[7] * m1 + R[8] * m2 + t[2];
-    const float opacity = opacities[i];
+    const float opacity = rows ? sO[row] : opacities[i];
     bool ok = !(z < cam.near_plane || z > cam.far_plane);
     if (ok) {
         float Rq[9];
         {
-            const float4 q = reinterpret_cast<const float4*>(quats)[i];
+            const float4 q = rows ? sQ[row] : reinterpret_cast<const float4*>(quats)[i];
             const float inv = 1.0f / sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w);
             quat_to_rotmat(q.x * inv, q.y * inv, q.z * inv, q.w * inv, Rq);
         }
-        const float s[3] = {scales[3 * i], scales[3 * i + 1], scales[3 * i + 2]};
+        const float s[3] = {rows ? sS[3 * row] : scales[3 * i], rows ? sS[3 * row + 1] : scales[3 * i + 1],
+                            rows ? sS[3 * row + 2] : scales[3 * i + 2]};
         float M[9], Sigma[9], RS[9], Sc[9];
         world_cov(Rq, s, M, Sigma);
         cam_cov(R, Sigma, RS, Sc);
@@ -153,11 +185,19 @@ project_fwd_kernel(int N, int C, const float* __restrict__ means, const float* _
         float inv = 1.0f / sqrtf(dx * dx + dy * dy + dz * dz);
         float B[16];
         sh_basis(sh_degree, dx * inv, dy * inv, dz * inv, B);
-        float c48[48];
-        load_sh_coeffs(sh, i, C, c48);          // C > 1: the chunk's C view warps read the same lines
+        if (rows) {
+            const float* sc = sSH + row * SH_ROW;
 #pragma unroll
-        for (int k = 0; k < 16; ++k) {
-            r += B[k] * c48[3 * k]; g += B[k] * c48[3 * k + 1]; bl += B[k] * c48[3 * k + 2];
+            for (int k = 0; k < 16; ++k) {
+                r += B[k] * sc[3 * k]; g += B[k] * sc[3 * k + 1]; bl += B[k] * sc[3 * k + 2];
+            }
+        } else {
+            float c48[48];
+            load_sh_coeffs(sh, i, C, c48);      // C > 1: the chunk's C view warps read the same lines
+#pragma unroll
+            for (int k = 0; k < 16; ++k) {
+                r += B[k] * c48[3 * k]; g += B[k] * c48[3 * k + 1]; bl += B[k] * c48[3 * k + 2];
+            }
         }
         r = fmaxf(r + 0.5f, 0.f); g = fmaxf(g + 0.5f, 0.f); bl = fmaxf(bl + 0.5f, 0.f);
     }
@@ -197,7 +237,15 @@ static int project_fwd_impl(const char* name, int convention, int N, int C, cons
     const long long warps = (long long)adb_cdiv(N, 32) * C;
     if (warps >= (1LL << 32) - PROJ_WARPS || N > 2147483647 - 32) return refuse(name, "too many (Gaussian, view) pairs");
     const unsigned blocks = (unsigned)((warps + PROJ_WARPS - 1) / PROJ_WARPS);
-    project_fwd_kernel<<<blocks, PROJ_WARPS * 32, 0, stream>>>(N, C, means, quats, scales, opacities, sh, sh_degree, cam,
+    constexpr int max_smem = proj_rows(1) * PROJ_ROW_FLOATS * (int)sizeof(float);     // 63 KB: above the 48 KB default
+    static AdbDeviceOnce once;
+    const int rc = once.ensure([]() -> int {
+        ADB_CUDA(cudaFuncSetAttribute(project_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+        return ADB_OK;
+    });
+    if (rc != ADB_OK) return rc;
+    const size_t smem = (size_t)proj_rows(C) * PROJ_ROW_FLOATS * sizeof(float);
+    project_fwd_kernel<<<blocks, PROJ_WARPS * 32, smem, stream>>>(N, C, means, quats, scales, opacities, sh, sh_degree, cam,
                                                               radii, splats, tiles_per_gauss, tile_counts);
     ADB_CHECK_LAUNCH("project_fwd_kernel");
     return ADB_OK;

@@ -176,20 +176,19 @@ sh_bwd_multi_kernel(int N, int C, const float* __restrict__ means, const float* 
                     float* __restrict__ v_means, int accumulate, int skip_mod, int skip_val,
                     float* __restrict__ v_campos) {
     __shared__ float sRed[PB / 32][3];
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    // the CTA's SH rows, staged with coalesced copies (raster_geom.cuh); after the views each thread's row takes its v_sh
+    __shared__ __align__(16) float sRows[PB * SH_ROW];
+    const int first = blockIdx.x * PB, n = min(PB, N - first);
+    stage_sh_rows(sRows, sh, first, n);
+    const int i = first + threadIdx.x;
     const bool in = i < N;
+    float* const row = sRows + threadIdx.x * SH_ROW;
     float mu[3] = {0.f, 0.f, 0.f};
-    float c48[48], o48[48];
+    float o48[48];
 #pragma unroll
-    for (int k = 0; k < 48; ++k) { c48[k] = 0.f; o48[k] = 0.f; }
+    for (int k = 0; k < 48; ++k) o48[k] = 0.f;
     if (in) {
         mu[0] = means[3 * i]; mu[1] = means[3 * i + 1]; mu[2] = means[3 * i + 2];
-        const float4* sp = reinterpret_cast<const float4*>(sh + (size_t)i * 48);
-#pragma unroll
-        for (int k = 0; k < 12; ++k) {
-            const float4 q = adb_ldg_stream4(sp + k);
-            c48[4 * k] = q.x; c48[4 * k + 1] = q.y; c48[4 * k + 2] = q.z; c48[4 * k + 3] = q.w;
-        }
         if (accumulate & 2) {            // second pass of a split expansion: continue from the stored partial sums
             const float4* op0 = reinterpret_cast<const float4*>(v_sh + (size_t)i * 48);
 #pragma unroll
@@ -199,6 +198,8 @@ sh_bwd_multi_kernel(int N, int C, const float* __restrict__ means, const float* 
             }
         }
     }
+    cp_async_wait_all();
+    __syncthreads();
     float gm[3] = {0.f, 0.f, 0.f};
     // software pipeline: the colour gradient of view c+1 is in flight while view c is expanded.  (A two-lanes-per-Gaussian
     // split of the 16 coefficients duplicates the basis evaluation, which costs more than the halved register footprint buys.)
@@ -225,7 +226,7 @@ sh_bwd_multi_kernel(int N, int C, const float* __restrict__ means, const float* 
 #pragma unroll
             for (int k = 0; k < 16; ++k) {
                 // s_k = <coefficients of band k, g>: one dot product feeds the three direction-gradient sums
-                const float sk = fmaf(c48[3 * k], g[0], fmaf(c48[3 * k + 1], g[1], c48[3 * k + 2] * g[2]));
+                const float sk = fmaf(row[3 * k], g[0], fmaf(row[3 * k + 1], g[1], row[3 * k + 2] * g[2]));
                 vnx = fmaf(Bx[k], sk, vnx); vny = fmaf(By[k], sk, vny); vnz = fmaf(Bz[k], sk, vnz);
                 o48[3 * k] = fmaf(Bs[k], g[0], o48[3 * k]);
                 o48[3 * k + 1] = fmaf(Bs[k], g[1], o48[3 * k + 1]);
@@ -251,10 +252,13 @@ sh_bwd_multi_kernel(int N, int C, const float* __restrict__ means, const float* 
             }
         }
     }
-    if (!in) return;
-    float4* op = reinterpret_cast<float4*>(v_sh + (size_t)i * 48);
+    // v_sh through the thread's own (no longer read) row, then coalesced row stores
 #pragma unroll
-    for (int k = 0; k < 12; ++k) op[k] = make_float4(o48[4 * k], o48[4 * k + 1], o48[4 * k + 2], o48[4 * k + 3]);
+    for (int k = 0; k < 12; ++k)
+        reinterpret_cast<float4*>(row)[k] = make_float4(o48[4 * k], o48[4 * k + 1], o48[4 * k + 2], o48[4 * k + 3]);
+    __syncthreads();
+    store_sh_rows(v_sh, sRows, first, n);
+    if (!in) return;
     if (accumulate & 1) { v_means[3 * i] += gm[0]; v_means[3 * i + 1] += gm[1]; v_means[3 * i + 2] += gm[2]; }
     else                { v_means[3 * i] = gm[0];  v_means[3 * i + 1] = gm[1];  v_means[3 * i + 2] = gm[2]; }
 }
@@ -271,35 +275,40 @@ sh_bwd_multi_kernel(int N, int C, const float* __restrict__ means, const float* 
 __global__ void __launch_bounds__(PB)
 sh_expand_multi_kernel(int N, int C, const float* __restrict__ means, int sh_degree, const float* __restrict__ campos,
                        const float* __restrict__ g_rgb, float* __restrict__ v_sh) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= N) return;
-    const float mx = means[3 * i], my = means[3 * i + 1], mz = means[3 * i + 2];
-    float o48[48];
+    __shared__ __align__(16) float sRows[PB * SH_ROW];      // v_sh rows, stored coalesced (raster_geom.cuh)
+    const int first = blockIdx.x * PB, n = min(PB, N - first);
+    const int i = first + threadIdx.x;
+    if (i < N) {
+        const float mx = means[3 * i], my = means[3 * i + 1], mz = means[3 * i + 2];
+        float o48[48];
 #pragma unroll
-    for (int k = 0; k < 48; ++k) o48[k] = 0.f;
-    const float* gp = g_rgb + (size_t)i * 3;
-    float gn0 = gp[0], gn1 = gp[1], gn2 = gp[2];
-    for (int c = 0; c < C; ++c) {
-        const float g0 = gn0, g1 = gn1, g2 = gn2;
-        if (c + 1 < C) {                                  // next view's colour gradient in flight while this one is expanded
-            const float* gq = g_rgb + ((size_t)(c + 1) * N + i) * 3;
-            gn0 = gq[0]; gn1 = gq[1]; gn2 = gq[2];
-        }
-        if (g0 == 0.f && g1 == 0.f && g2 == 0.f) continue;
-        const float dx = mx - campos[3 * c], dy = my - campos[3 * c + 1], dz = mz - campos[3 * c + 2];
-        const float inv = rsqrtf(dx * dx + dy * dy + dz * dz);
-        float Bs[16];
-        sh_basis(sh_degree, dx * inv, dy * inv, dz * inv, Bs);
+        for (int k = 0; k < 48; ++k) o48[k] = 0.f;
+        const float* gp = g_rgb + (size_t)i * 3;
+        float gn0 = gp[0], gn1 = gp[1], gn2 = gp[2];
+        for (int c = 0; c < C; ++c) {
+            const float g0 = gn0, g1 = gn1, g2 = gn2;
+            if (c + 1 < C) {                              // next view's colour gradient in flight while this one is expanded
+                const float* gq = g_rgb + ((size_t)(c + 1) * N + i) * 3;
+                gn0 = gq[0]; gn1 = gq[1]; gn2 = gq[2];
+            }
+            if (g0 == 0.f && g1 == 0.f && g2 == 0.f) continue;
+            const float dx = mx - campos[3 * c], dy = my - campos[3 * c + 1], dz = mz - campos[3 * c + 2];
+            const float inv = rsqrtf(dx * dx + dy * dy + dz * dz);
+            float Bs[16];
+            sh_basis(sh_degree, dx * inv, dy * inv, dz * inv, Bs);
 #pragma unroll
-        for (int k = 0; k < 16; ++k) {
-            o48[3 * k] = fmaf(Bs[k], g0, o48[3 * k]);
-            o48[3 * k + 1] = fmaf(Bs[k], g1, o48[3 * k + 1]);
-            o48[3 * k + 2] = fmaf(Bs[k], g2, o48[3 * k + 2]);
+            for (int k = 0; k < 16; ++k) {
+                o48[3 * k] = fmaf(Bs[k], g0, o48[3 * k]);
+                o48[3 * k + 1] = fmaf(Bs[k], g1, o48[3 * k + 1]);
+                o48[3 * k + 2] = fmaf(Bs[k], g2, o48[3 * k + 2]);
+            }
         }
+        float4* op = reinterpret_cast<float4*>(sRows + threadIdx.x * SH_ROW);
+#pragma unroll
+        for (int k = 0; k < 12; ++k) op[k] = make_float4(o48[4 * k], o48[4 * k + 1], o48[4 * k + 2], o48[4 * k + 3]);
     }
-    float4* op = reinterpret_cast<float4*>(v_sh + (size_t)i * 48);
-#pragma unroll
-    for (int k = 0; k < 12; ++k) op[k] = make_float4(o48[4 * k], o48[4 * k + 1], o48[4 * k + 2], o48[4 * k + 3]);
+    __syncthreads();
+    store_sh_rows(v_sh, sRows, first, n);
 }
 
 // v_means[i] += sum over the LOCAL views of the colour gradient pulled back through the view direction; v_campos[c] gets the
@@ -310,21 +319,16 @@ sh_dir_bwd_multi_kernel(int N, int C, const float* __restrict__ means, const flo
                         const float* __restrict__ campos, const float* __restrict__ splats, const float* __restrict__ v_splats,
                         float* __restrict__ v_means, float* __restrict__ v_campos) {
     __shared__ float sRed[PB / 32][3];
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    __shared__ __align__(16) float sRows[PB * SH_ROW];      // the CTA's SH rows, staged coalesced (raster_geom.cuh)
+    const int first = blockIdx.x * PB, n = min(PB, N - first);
+    stage_sh_rows(sRows, sh, first, n);
+    const int i = first + threadIdx.x;
     const bool in = i < N;
+    const float* const row = sRows + threadIdx.x * SH_ROW;
     float mu[3] = {0.f, 0.f, 0.f};
-    float c48[48];
-#pragma unroll
-    for (int k = 0; k < 48; ++k) c48[k] = 0.f;
-    if (in) {
-        mu[0] = means[3 * i]; mu[1] = means[3 * i + 1]; mu[2] = means[3 * i + 2];
-        const float4* sp = reinterpret_cast<const float4*>(sh + (size_t)i * 48);
-#pragma unroll
-        for (int k = 0; k < 12; ++k) {
-            const float4 q = adb_ldg_stream4(sp + k);
-            c48[4 * k] = q.x; c48[4 * k + 1] = q.y; c48[4 * k + 2] = q.z; c48[4 * k + 3] = q.w;
-        }
-    }
+    if (in) { mu[0] = means[3 * i]; mu[1] = means[3 * i + 1]; mu[2] = means[3 * i + 2]; }
+    cp_async_wait_all();
+    __syncthreads();
     float gm[3] = {0.f, 0.f, 0.f};
     for (int c = 0; c < C; ++c) {
         float red[3] = {0.f, 0.f, 0.f};
@@ -347,7 +351,7 @@ sh_dir_bwd_multi_kernel(int N, int C, const float* __restrict__ means, const flo
             float vnx = 0.f, vny = 0.f, vnz = 0.f;
 #pragma unroll
             for (int k = 0; k < 16; ++k) {
-                const float sk = fmaf(c48[3 * k], g[0], fmaf(c48[3 * k + 1], g[1], c48[3 * k + 2] * g[2]));
+                const float sk = fmaf(row[3 * k], g[0], fmaf(row[3 * k + 1], g[1], row[3 * k + 2] * g[2]));
                 vnx = fmaf(Bx[k], sk, vnx); vny = fmaf(By[k], sk, vny); vnz = fmaf(Bz[k], sk, vnz);
             }
             const float dot = vnx * nx + vny * ny + vnz * nz;

@@ -504,15 +504,16 @@ def multi_view_backward(means, quats, scales, sh, sh_degree, viewmats, Ks, campo
     v_campos = torch.zeros(Cn, 3, dtype=torch.float32, device=dev)
     Vc, Kc, Pc = _f32c(viewmats.detach()), _f32c(Ks.detach()), _f32c(camposs.detach())
     # colour gradient masked by the SH clamp (rgb = max(.,0): zero gradient where the record's colour is 0); invisible
-    # Gaussians have zero accumulators.  Produced first so that its all-gather overlaps the geometry kernel.
+    # Gaussians have zero accumulators.  One process: the geometry kernel writes it as it reads the same two records
+    # (bit for bit mask_rgb_grad).  Multi-GPU: produced first so that its all-gather overlaps the geometry kernel.
     g_rgb = out.get("g_rgb")
     if exchange is not None and getattr(exchange, "gather_started", False):
         pass                                      # per-view gathers were issued as each view's blend backward finished
     else:
         if g_rgb is None:
             g_rgb = torch.empty(Cn, N, 3, dtype=torch.float32, device=dev)
-        mask_rgb_grad(splats, v_splats, g_rgb)
         if exchange is not None:
+            mask_rgb_grad(splats, v_splats, g_rgb)
             exchange.start_gather(g_rgb, Pc)
     # an exchange with separate input / result buffers (peer.PeerExchange): the kernel writes this rank's partial sums into
     # `views_in`, the reduced gradients appear in `views`
@@ -521,7 +522,8 @@ def multi_view_backward(means, quats, scales, sh, sh_degree, viewmats, Ks, campo
         (v_means, v_quats, v_scales, v_opac)
     _lib.call("adb_raster_project_bwd_multi", N, Cn, _lib.ptr(means), _lib.ptr(quats), _lib.ptr(scales), _lib.ptr(Vc),
               _lib.ptr(Kc), W, H, _lib.ptr(radii), _lib.ptr(splats), _lib.ptr(v_splats), _lib.ptr(pm),
-              _lib.ptr(pq), _lib.ptr(ps), _lib.ptr(po), None, _lib.ptr(v_views), _lib.stream())
+              _lib.ptr(pq), _lib.ptr(ps), _lib.ptr(po), _lib.ptr(g_rgb) if exchange is None else None, _lib.ptr(v_views),
+              _lib.stream())
     if gin is not None:
         gout = exchange.views
         v_means, v_quats, v_scales, v_opac = gout["v_means"], gout["v_quats"], gout["v_scales"], gout["v_opac"]
