@@ -84,6 +84,7 @@ LAUNCHES = {
     "adb_raster_sh_expand_multi": 1, "adb_raster_project_fwd_counts": 1, "adb_raster_tile_scan": 1,
     "adb_raster_project_fwd_multi": 1, "adb_raster_tile_scan_multi": 1, "adb_raster_tile_scatter_sort_multi": 2,
     "adb_raster_blend_fwd_multi": 1, "adb_raster_blend_bwd_multi": 1,
+    "adb_raster_tile_band_scatter_sort": 3, "adb_raster_tile_band_scatter_sort_multi": 3,
 }
 
 

@@ -176,6 +176,19 @@ ADB_API int adb_raster_tile_offsets(long long n_isect, const int64_t* keys_sorte
 // COPIES = 4 replicas of every tile counter (selected by CTA index) cut the same-address serialisation of the L2 atomics
 // that a single counter per tile suffers.
 //
+// Band scatter (adb_raster_tile_band_scatter_sort*, what raster.intersect / intersect_multi run): the scatter above does
+// one returning L2 atomic and one stray 8-byte store per intersection, each to a random place, and its time follows the
+// number of those L2 requests rather than the bytes.  The band scatter replaces it by two passes whose stores leave
+// shared memory as runs of consecutive slots:
+//   band pass  per chunk of 2048 Gaussians: one pair (word, x0 | x1 << 16) per tile row the rectangle touches, counted per
+//              row in shared memory, one global atomic per (CTA, row) on the row's cursor, pairs grouped by row in shared
+//              memory and written as one run per row into the row's region of the scratch (the row's tile segments);
+//   tile pass  one CTA per (row, view): tile cursors in shared memory; per chunk of 1024 pairs the expanded words are
+//              grouped by tile in shared memory and written as one run per tile into `packed`;
+//   sort       tile_sort_kernel as above.
+// Each tile receives the same words as from the scatter, so the sorted output is the same bit for bit.  The per-(tile,
+// copy) counters are read only by the scan; the band scatter uses one cursor per row.
+//
 // Views: the scan, scatter and sort take C views at once (one scan CTA per view, a view grid dimension for the scatter,
 // (T, C) CTAs for the sort).  View c has its own counter block [2*COPIES*T] and tile_offsets row [T+1], and owns the segment
 // [base_c, base_c + cap_c) of the one packed/keys/vals buffer, base_c = sum of the previous views' capacities.  Offsets and
@@ -503,6 +516,290 @@ tile_sort_kernel(int T, const int32_t* __restrict__ offsets_all, u64* __restrict
     }
 }
 
+// ---- band scatter: (Gaussian, tile row) pairs appended in runs, then expanded into the tiles by one CTA per row ----------
+constexpr int BAND_THREADS = 256;
+constexpr int BAND_PER = 8;             // Gaussians per thread, held in registers between the counting and the writing pass
+constexpr int EXPAND_THREADS = 512;
+constexpr int EXPAND_PER = 2;           // pairs per thread per chunk, loaded before any of them is expanded
+constexpr int STAGE = 4096;             // entries a CTA stages in shared memory, grouped by row / tile, before writing them
+constexpr int MAX_BAND_TILES = 4096;    // tile rows and columns (W, H <= 65536): x0 | x1 << 16 fits a pair's column word
+
+// The splat's tile rectangle and its sort word; false when it has no tiles.  All four loads are issued before any of
+// them is tested, so that a thread's Gaussians have their loads in flight together.
+__device__ __forceinline__ bool band_splat(size_t vi, int i, const int32_t* __restrict__ radii,
+                                           const float* __restrict__ splats, const int32_t* __restrict__ tiles_per_gauss,
+                                           int W, int H, int convention, int& x0, int& x1, int& y0, int& y1, u64& word) {
+    const int tiles = __ldg(tiles_per_gauss + vi);
+    const int2 r = __ldg(reinterpret_cast<const int2*>(radii) + vi);
+    const float2 m = __ldg(reinterpret_cast<const float2*>(splats + vi * ADB_SPLAT_STRIDE));
+    const float depth = __ldg(splats + vi * ADB_SPLAT_STRIDE + 11);
+    adb_tile_rect(m.x, m.y, r.x, r.y, W, H, convention, x0, x1, y0, y1);
+    word = ((u64)__float_as_uint(depth) << 32) | (unsigned)i;
+    return tiles > 0 && x0 < x1 && y0 < y1;
+}
+
+// A warp's runs spread over its lanes: lane p owns the items [lo_p, lo_p + n_p), and f(p, v) runs once for every item v
+// of every lane p, 32 items at a time (lane j takes item j of the warp's concatenated runs, found by a binary search of the
+// run starts), so that one wide splat does not hold up the other 31 lanes.  All 32 lanes call it with the same `s`.
+struct WarpRuns {
+    unsigned lo[32], excl[32];
+};
+
+template <class F>
+__device__ __forceinline__ void warp_runs(WarpRuns& s, int lane, unsigned lo, unsigned n, F&& f) {
+    unsigned incl = n;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned y = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += y;
+    }
+    const unsigned total = __shfl_sync(0xffffffffu, incl, 31);
+    s.lo[lane] = lo;
+    s.excl[lane] = incl - n;
+    __syncwarp();
+    for (unsigned j = lane; j < total; j += 32) {
+        int p = 0;                                  // the last lane whose run starts at or before item j
+#pragma unroll
+        for (int step = 16; step > 0; step >>= 1)
+            if (s.excl[p + step] <= j) p += step;
+        f(p, s.lo[p] + (j - s.excl[p]));
+    }
+    __syncwarp();
+}
+
+// Exclusive scan of cnt[0..n) into loc (cnt is zeroed); returns the total.  Each thread owns a contiguous range of entries.
+// s_part: THREADS / 32 words.  Ends with a barrier.
+template <int THREADS>
+__device__ __forceinline__ unsigned block_scan(unsigned* cnt, unsigned* loc, int n, unsigned* s_part) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, per = (n + THREADS - 1) / THREADS;
+    const int lo = min(n, tid * per), hi = min(n, lo + per);
+    unsigned sum = 0;
+    for (int e = lo; e < hi; ++e) sum += cnt[e];
+    unsigned incl = sum;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned y = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += y;
+    }
+    if (lane == 31) s_part[warp] = incl;
+    __syncthreads();
+    if (warp == 0) {
+        unsigned v = lane < THREADS / 32 ? s_part[lane] : 0;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned y = __shfl_up_sync(0xffffffffu, v, o);
+            if (lane >= o) v += y;
+        }
+        if (lane < THREADS / 32) s_part[lane] = v;
+    }
+    __syncthreads();
+    unsigned run = (warp ? s_part[warp - 1] : 0) + incl - sum;
+    for (int e = lo; e < hi; ++e) {
+        loc[e] = run;
+        run += cnt[e];
+        cnt[e] = 0;
+    }
+    const unsigned total = s_part[THREADS / 32 - 1];
+    __syncthreads();
+    return total;
+}
+
+// Band pass.  Grid (Gaussian chunks of BAND_THREADS * BAND_PER, views).  Each CTA counts its pairs per tile row in shared
+// memory, reserves one run per row with one global atomic on the row's cursor, then writes its pairs into those runs.
+// Row b's region of the pair arrays is its tiles' segment [offsets[b*tw], offsets[(b+1)*tw]): a row has at most as many
+// pairs as intersections, so the region holds them unless the capacity cut it (pairs past its end are dropped here and
+// rebuilt by the tile pass).  The cursor of row b is the scan's segment start of (tile b*tw, copy 0), which equals
+// offsets[b*tw]; it counts every pair of the row, kept or not, and stays below 2^32 (at most N pairs per row).
+__global__ void __launch_bounds__(BAND_THREADS)
+tile_band_kernel(int N, const int32_t* __restrict__ radii, const float* __restrict__ splats,
+                 const int32_t* __restrict__ tiles_per_gauss, int W, int H, int convention, int32_t* __restrict__ counts_all,
+                 const int32_t* __restrict__ offsets_all, u64* __restrict__ pair_words, uint32_t* __restrict__ pair_cols) {
+    extern __shared__ u64 s_band[];
+    __shared__ WarpRuns s_runs[BAND_THREADS / 32];
+    __shared__ u64 s_word[BAND_THREADS];
+    __shared__ uint32_t s_cols[BAND_THREADS];
+    __shared__ unsigned s_part[BAND_THREADS / 32];
+    const int tw = (W + ADB_TILE - 1) / ADB_TILE, th = (H + ADB_TILE - 1) / ADB_TILE, T = tw * th;
+    u64* s_stage_w = s_band;                                            // [STAGE] the CTA's pairs grouped by row
+    uint32_t* s_stage_c = reinterpret_cast<uint32_t*>(s_band + STAGE);  // [STAGE]
+    uint16_t* s_stage_b = reinterpret_cast<uint16_t*>(s_stage_c + STAGE);   // [STAGE] their rows
+    unsigned* s_cnt = reinterpret_cast<unsigned*>(s_stage_b + STAGE);   // pairs per row, then the rank inside the run
+    unsigned* s_base = s_cnt + th;              // the run's first slot
+    unsigned* s_end = s_cnt + 2 * th;           // the row region's end
+    unsigned* s_loc = s_cnt + 3 * th;           // the run's first entry in the stage
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, view = blockIdx.y;
+    unsigned* cursors = reinterpret_cast<unsigned*>(counts_all + (size_t)view * 2 * COPIES * T + (size_t)T * COPIES);
+    const int32_t* offsets = offsets_all + (size_t)view * (T + 1);
+    for (int b = tid; b < th; b += BAND_THREADS) s_cnt[b] = 0;
+    __syncthreads();
+    uint32_t cols[BAND_PER], rows[BAND_PER];
+    u64 words[BAND_PER];
+    const int g0 = blockIdx.x * BAND_THREADS * BAND_PER + tid;
+#pragma unroll
+    for (int k = 0; k < BAND_PER; ++k) {
+        const int i = g0 + k * BAND_THREADS;
+        int x0 = 0, x1 = 0, y0 = 0, y1 = 0;
+        words[k] = 0;
+        if (i >= N || !band_splat((size_t)view * N + i, i, radii, splats, tiles_per_gauss, W, H, convention, x0, x1, y0, y1,
+                                  words[k]))
+            y0 = y1 = 0;
+        rows[k] = (uint32_t)y0 | ((uint32_t)y1 << 16);
+        cols[k] = (uint32_t)x0 | ((uint32_t)x1 << 16);
+    }
+#pragma unroll
+    for (int k = 0; k < BAND_PER; ++k) {
+        const unsigned y0 = rows[k] & 0xffffu, y1 = rows[k] >> 16;
+        warp_runs(s_runs[warp], lane, y0, y1 - y0, [&](int, unsigned b) { atomicAdd(s_cnt + b, 1u); });
+    }
+    __syncthreads();
+    for (int b = tid; b < th; b += BAND_THREADS) {
+        const unsigned n = s_cnt[b];
+        if (n) {
+            s_base[b] = atomicAdd(cursors + (size_t)b * tw * COPIES, n);
+            s_end[b] = (unsigned)offsets[(b + 1) * tw];
+        }
+    }
+    const unsigned K = block_scan<BAND_THREADS>(s_cnt, s_loc, th, s_part);
+    u64* my_word = s_word + warp * 32;
+    uint32_t* my_cols = s_cols + warp * 32;
+    const bool staged = K <= STAGE;             // else (many rows per splat) each pair is stored where it lands
+#pragma unroll
+    for (int k = 0; k < BAND_PER; ++k) {
+        const unsigned y0 = rows[k] & 0xffffu, y1 = rows[k] >> 16;
+        my_word[lane] = words[k];
+        my_cols[lane] = cols[k];
+        warp_runs(s_runs[warp], lane, y0, y1 - y0, [&](int p, unsigned b) {
+            const unsigned r = atomicAdd(s_cnt + b, 1u);
+            if (staged) {
+                const unsigned q = s_loc[b] + r;
+                s_stage_w[q] = my_word[p];
+                s_stage_c[q] = my_cols[p];
+                s_stage_b[q] = (uint16_t)b;
+            } else if (s_base[b] + r < s_end[b]) {
+                pair_words[s_base[b] + r] = my_word[p];
+                pair_cols[s_base[b] + r] = my_cols[p];
+            }
+        });
+    }
+    if (!staged) return;
+    __syncthreads();
+    for (unsigned q = tid; q < K; q += BAND_THREADS) {   // consecutive entries of a row go to consecutive slots
+        const unsigned b = s_stage_b[q], slot = s_base[b] + (q - s_loc[b]);
+        if (slot < s_end[b]) {
+            pair_words[slot] = s_stage_w[q];
+            pair_cols[slot] = s_stage_c[q];
+        }
+    }
+}
+
+// Tile pass.  Grid (tile rows, views).  The row's tile cursors live in shared memory, seeded from offsets; the CTA streams
+// the row's pairs, expands each over its columns [x0, x1) (a shared-memory atomic per tile gives the slot in the tile's
+// segment) and so writes each tile's words as runs of consecutive slots.  It also zeroes the row's counters (the first
+// half of tile_counts), so they are zero again after the call.  When the capacity cut the row's region below its pair
+// count, the kept pairs are not all the row's pairs: the CTA then rebuilds the row's pairs from the splats instead, so
+// that every tile the capacity leaves whole is complete and every slot of the region is written.
+__global__ void __launch_bounds__(EXPAND_THREADS)
+tile_expand_kernel(int N, const int32_t* __restrict__ radii, const float* __restrict__ splats,
+                   const int32_t* __restrict__ tiles_per_gauss, int W, int H, int convention,
+                   int32_t* __restrict__ counts_all, const int32_t* __restrict__ offsets_all,
+                   const u64* __restrict__ pair_words, const uint32_t* __restrict__ pair_cols, u64* __restrict__ packed) {
+    extern __shared__ u64 s_tiles[];
+    __shared__ WarpRuns s_runs[EXPAND_THREADS / 32];
+    __shared__ u64 s_word[EXPAND_THREADS];
+    __shared__ unsigned s_part[EXPAND_THREADS / 32];
+    const int tw = (W + ADB_TILE - 1) / ADB_TILE, T = tw * ((H + ADB_TILE - 1) / ADB_TILE);
+    u64* s_stage_w = s_tiles;                                                       // [STAGE] a chunk's words by tile
+    uint16_t* s_stage_x = reinterpret_cast<uint16_t*>(s_tiles + STAGE);             // [STAGE] their tile columns
+    unsigned* s_cur = reinterpret_cast<unsigned*>(s_stage_x + STAGE);               // next slot of each tile
+    unsigned* s_end = s_cur + tw;                                                   // end of each tile's segment
+    unsigned* s_cnt = s_cur + 2 * tw;                                               // a chunk's words per tile
+    unsigned* s_loc = s_cur + 3 * tw;                                               // their first entry in the stage
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, band = blockIdx.x, view = blockIdx.y, t0 = band * tw;
+    int32_t* counts = counts_all + (size_t)view * 2 * COPIES * T;
+    const int32_t* offsets = offsets_all + (size_t)view * (T + 1);
+    for (int x = tid; x < tw; x += EXPAND_THREADS) {
+        s_cur[x] = (unsigned)offsets[t0 + x];
+        s_end[x] = (unsigned)offsets[t0 + x + 1];
+        s_cnt[x] = 0;
+    }
+    for (int e = tid; e < tw * COPIES; e += EXPAND_THREADS) counts[(size_t)t0 * COPIES + e] = 0;
+    const unsigned start = (unsigned)offsets[t0], end = (unsigned)offsets[t0 + tw];
+    const unsigned pairs_end = reinterpret_cast<const unsigned*>(counts + (size_t)T * COPIES)[(size_t)t0 * COPIES];
+    __syncthreads();
+    if (start == end) return;
+    u64* my_word = s_word + warp * 32;
+    auto expand = [&](int p, unsigned x) {
+        const unsigned slot = atomicAdd(s_cur + x, 1u);
+        if (slot < s_end[x]) packed[slot] = my_word[p];
+    };
+    if (pairs_end <= end) {
+        const int n = (int)(pairs_end - start);
+        for (int p0 = 0; p0 < n; p0 += EXPAND_THREADS * EXPAND_PER) {
+            u64 w[EXPAND_PER];
+            uint32_t c[EXPAND_PER];
+#pragma unroll
+            for (int k = 0; k < EXPAND_PER; ++k) {
+                const int p = p0 + k * EXPAND_THREADS + tid;
+                w[k] = 0;
+                c[k] = 0;
+                if (p < n) {
+                    w[k] = pair_words[start + p];
+                    c[k] = pair_cols[start + p];
+                }
+            }
+#pragma unroll
+            for (int k = 0; k < EXPAND_PER; ++k) {
+                const unsigned x0 = c[k] & 0xffffu, x1 = c[k] >> 16;
+                warp_runs(s_runs[warp], lane, x0, x1 - x0, [&](int, unsigned x) { atomicAdd(s_cnt + x, 1u); });
+            }
+            __syncthreads();
+            const unsigned K = block_scan<EXPAND_THREADS>(s_cnt, s_loc, tw, s_part);
+            if (K > STAGE) {                        // wide pairs: this chunk stores each word where it lands
+#pragma unroll
+                for (int k = 0; k < EXPAND_PER; ++k) {
+                    const unsigned x0 = c[k] & 0xffffu, x1 = c[k] >> 16;
+                    my_word[lane] = w[k];
+                    warp_runs(s_runs[warp], lane, x0, x1 - x0, expand);
+                }
+                __syncthreads();
+                continue;
+            }
+#pragma unroll
+            for (int k = 0; k < EXPAND_PER; ++k) {
+                const unsigned x0 = c[k] & 0xffffu, x1 = c[k] >> 16;
+                my_word[lane] = w[k];
+                warp_runs(s_runs[warp], lane, x0, x1 - x0, [&](int p, unsigned x) {
+                    const unsigned q = s_loc[x] + atomicAdd(s_cnt + x, 1u);
+                    s_stage_w[q] = my_word[p];
+                    s_stage_x[q] = (uint16_t)x;
+                });
+            }
+            __syncthreads();
+            for (unsigned q = tid; q < K; q += EXPAND_THREADS) {   // consecutive entries of a tile: consecutive slots
+                const unsigned x = s_stage_x[q], slot = s_cur[x] + (q - s_loc[x]);
+                if (slot < s_end[x]) packed[slot] = s_stage_w[q];
+            }
+            __syncthreads();
+            for (int x = tid; x < tw; x += EXPAND_THREADS) {
+                s_cur[x] += s_cnt[x];
+                s_cnt[x] = 0;
+            }
+            __syncthreads();
+        }
+    } else {
+        for (int i0 = 0; i0 < N; i0 += EXPAND_THREADS) {
+            const int i = i0 + tid;
+            int x0 = 0, x1 = 0, y0 = 0, y1 = 0;
+            u64 w = 0;
+            const bool mine = i < N &&
+                band_splat((size_t)view * N + i, i, radii, splats, tiles_per_gauss, W, H, convention, x0, x1, y0, y1, w) &&
+                y0 <= band && band < y1;
+            my_word[lane] = w;
+            warp_runs(s_runs[warp], lane, x0, mine ? x1 - x0 : 0, expand);
+        }
+    }
+}
+
 }  // namespace
 
 // Fills the per-view segments from the host array of capacities; refuses what the int32 offsets cannot address.
@@ -639,4 +936,86 @@ ADB_API int adb_raster_tile_scatter_sort_multi(int N, int C, const int32_t* radi
                 "adb_raster_tile_scatter_sort_multi: null pointer");
     return scatter_sort_launch(N, C, radii, splats, tiles_per_gauss, W, H, ADB_CONV_GSPLAT, 0, seg, tile_counts, tile_offsets,
                                packed, keys, vals, stream);
+}
+
+// Pair words (8 B) and pair columns (4 B) per slot of the intersection buffer.
+ADB_API int adb_raster_tile_band_scratch_bytes(long long capacity, size_t* bytes) {
+    ADB_REQUIRE(bytes && capacity >= 0 && capacity < 2147483647LL, "adb_raster_tile_band_scratch_bytes: bad args");
+    *bytes = (size_t)capacity * (sizeof(unsigned long long) + sizeof(uint32_t));
+    return ADB_OK;
+}
+
+static int band_scatter_sort_launch(const char* name, int N, int C, const int32_t* radii, const float* splats,
+                                    const int32_t* tiles_per_gauss, int W, int H, int convention, int cam0,
+                                    long long capacity, int32_t* tile_counts, const int32_t* tile_offsets, void* packed,
+                                    void* scratch, size_t scratch_bytes, int64_t* keys, int32_t* vals, cudaStream_t stream) {
+    const int tw = adb_cdiv(W, ADB_TILE), th = adb_cdiv(H, ADB_TILE), T = tw * th;
+    char msg[160];
+    if (tw > MAX_BAND_TILES || th > MAX_BAND_TILES) {
+        snprintf(msg, sizeof(msg), "%s: W and H must be at most %d", name, MAX_BAND_TILES * ADB_TILE);
+        adb_set_error_msg(msg);
+        return ADB_ERR_INVALID;
+    }
+    size_t need = 0;
+    adb_raster_tile_band_scratch_bytes(capacity, &need);
+    if (scratch_bytes < need) {
+        snprintf(msg, sizeof(msg), "%s: scratch too small (%zu < %zu bytes)", name, scratch_bytes, need);
+        adb_set_error_msg(msg);
+        return ADB_ERR_WORKSPACE;
+    }
+    u64* pair_words = static_cast<u64*>(scratch);
+    uint32_t* pair_cols = reinterpret_cast<uint32_t*>(pair_words + capacity);
+    const size_t band_smem = STAGE * (sizeof(u64) + sizeof(uint32_t) + sizeof(uint16_t)) + 4 * th * sizeof(unsigned);
+    const size_t expand_smem = STAGE * (sizeof(u64) + sizeof(uint16_t)) + 4 * tw * sizeof(unsigned);
+    ADB_CUDA(cudaFuncSetAttribute(tile_band_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)band_smem));
+    ADB_CUDA(cudaFuncSetAttribute(tile_expand_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)expand_smem));
+    tile_band_kernel<<<dim3(adb_cdiv(N, BAND_THREADS * BAND_PER), C), BAND_THREADS, band_smem, stream>>>(
+        N, radii, splats, tiles_per_gauss, W, H, convention, tile_counts, tile_offsets, pair_words, pair_cols);
+    ADB_CHECK_LAUNCH("tile_band_kernel");
+    tile_expand_kernel<<<dim3(th, C), EXPAND_THREADS, expand_smem, stream>>>(
+        N, radii, splats, tiles_per_gauss, W, H, convention, tile_counts, tile_offsets, pair_words, pair_cols,
+        (u64*)packed);
+    ADB_CHECK_LAUNCH("tile_expand_kernel");
+    tile_sort_kernel<<<dim3(T, C), SORT_THREADS, 0, stream>>>(T, tile_offsets, (u64*)packed, cam0, N, adb_tile_bits(W, H),
+                                                             keys, vals);
+    ADB_CHECK_LAUNCH("tile_sort_kernel");
+    return ADB_OK;
+}
+
+// adb_raster_tile_scatter_sort with the band scatter; scratch from adb_raster_tile_band_scratch_bytes(capacity).
+ADB_API int adb_raster_tile_band_scatter_sort(int N, const int32_t* radii, const float* splats,
+                                              const int32_t* tiles_per_gauss, int W, int H, int legacy, int cam_id,
+                                              int n_cams, long long capacity, int32_t* tile_counts,
+                                              const int32_t* tile_offsets, void* packed, void* scratch,
+                                              size_t scratch_bytes, int64_t* keys, int32_t* vals, cudaStream_t stream) {
+    ADB_REQUIRE(N >= 0 && W > 0 && H > 0 && cam_id >= 0 && n_cams > cam_id && capacity >= 0,
+                "adb_raster_tile_band_scatter_sort: bad sizes");
+    if (N == 0 || capacity == 0) return ADB_OK;
+    ADB_REQUIRE(radii && splats && tiles_per_gauss && tile_counts && tile_offsets && packed && scratch && keys && vals,
+                "adb_raster_tile_band_scatter_sort: null pointer");
+    ADB_REQUIRE(capacity < 2147483647LL, "adb_raster_tile_band_scatter_sort: bad sizes");
+    return band_scatter_sort_launch("adb_raster_tile_band_scatter_sort", N, 1, radii, splats, tiles_per_gauss, W, H,
+                                    legacy ? ADB_CONV_INRIA : ADB_CONV_GSPLAT, cam_id, capacity, tile_counts, tile_offsets,
+                                    packed, scratch, scratch_bytes, keys, vals, stream);
+}
+
+// adb_raster_tile_scatter_sort_multi with the band scatter; scratch from adb_raster_tile_band_scratch_bytes(sum of the
+// capacities).
+ADB_API int adb_raster_tile_band_scatter_sort_multi(int N, int C, const int32_t* radii, const float* splats,
+                                                    const int32_t* tiles_per_gauss, int W, int H,
+                                                    const long long* capacities, int32_t* tile_counts,
+                                                    const int32_t* tile_offsets, void* packed, void* scratch,
+                                                    size_t scratch_bytes, int64_t* keys, int32_t* vals,
+                                                    cudaStream_t stream) {
+    Segments seg;
+    const int rc = make_segments("adb_raster_tile_band_scatter_sort_multi", C, capacities, seg);
+    if (rc != ADB_OK) return rc;
+    ADB_REQUIRE(N >= 0 && W > 0 && H > 0 && (long long)C * N < 2147483647LL,
+                "adb_raster_tile_band_scatter_sort_multi: bad sizes");
+    if (N == 0) return ADB_OK;
+    ADB_REQUIRE(radii && splats && tiles_per_gauss && tile_counts && tile_offsets && packed && scratch && vals,
+                "adb_raster_tile_band_scatter_sort_multi: null pointer");
+    return band_scatter_sort_launch("adb_raster_tile_band_scatter_sort_multi", N, C, radii, splats, tiles_per_gauss, W, H,
+                                    ADB_CONV_GSPLAT, 0, seg.base[C - 1] + seg.cap[C - 1], tile_counts, tile_offsets, packed,
+                                    scratch, scratch_bytes, keys, vals, stream);
 }

@@ -31,6 +31,9 @@ _lib.register("adb_raster_sort", [i64, i32, i32, i32, vp, vp, vp, vp, vp, C.c_si
 _lib.register("adb_raster_tile_offsets", [i64, vp, i32, i32, vp, vp])
 _lib.register("adb_raster_tile_count_scan", [i32, vp, vp, vp, i32, i32, i32, i64, vp, vp, vp, vp, vp])
 _lib.register("adb_raster_tile_scatter_sort", [i32, vp, vp, vp, i32, i32, i32, i32, i32, i64, vp, vp, vp, vp, vp, vp])
+_lib.register("adb_raster_tile_band_scratch_bytes", [i64, C.POINTER(C.c_size_t)])
+_lib.register("adb_raster_tile_band_scatter_sort", [i32, vp, vp, vp, i32, i32, i32, i32, i32, i64, vp, vp, vp, vp,
+                                                    C.c_size_t, vp, vp, vp])
 _lib.register("adb_raster_blend_fwd", [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp])
 _lib.register("adb_raster_blend_bwd", [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp])
 _lib.register("adb_raster_project_bwd", [i32, vp, vp, vp, vp, i32, vp, vp, vp, i32, i32, f32, f32, f32, f32,
@@ -54,6 +57,8 @@ _lib.register("adb_raster_project_fwd_multi", [i32, i32, vp, vp, vp, vp, vp, i32
                                                vp, vp, vp, vp, vp])
 _lib.register("adb_raster_tile_scan_multi", [i32, i32, i32, _caps_t, vp, vp, vp, vp, vp])
 _lib.register("adb_raster_tile_scatter_sort_multi", [i32, i32, vp, vp, vp, i32, i32, _caps_t, vp, vp, vp, vp, vp, vp])
+_lib.register("adb_raster_tile_band_scatter_sort_multi", [i32, i32, vp, vp, vp, i32, i32, _caps_t, vp, vp, vp, vp,
+                                                          C.c_size_t, vp, vp, vp])
 _lib.register("adb_raster_blend_fwd_multi", [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp])
 _lib.register("adb_raster_blend_bwd_multi", [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp])
 
@@ -139,6 +144,13 @@ def new_tile_counts(W, H, dev, views=None):
     return torch.zeros(shape, dtype=torch.int32, device=dev)
 
 
+def band_scratch(capacity, dev):
+    """Uninitialised scratch of the band scatter (adb_raster_tile_band_scatter_sort*) for ``capacity`` intersections."""
+    nb = C.c_size_t(0)
+    _lib.call("adb_raster_tile_band_scratch_bytes", int(capacity), C.byref(nb))
+    return torch.empty(max(nb.value, 1), dtype=torch.uint8, device=dev)
+
+
 # ---- the multi-view batch, stage by stage: one launch per stage for C views of the same Gaussians ----------------------------
 def project_multi(means, quats, scales, opacities, sh, sh_degree, viewmats, Ks, camposs, W, H, eps2d, near, far, radius_clip,
                   tile_counts, out=None):
@@ -159,9 +171,9 @@ def project_multi(means, quats, scales, opacities, sh, sh_degree, viewmats, Ks, 
 
 
 def intersect_multi(radii, splats, tpg, W, H, counts, capacities=None, keys=True, info=None):
-    """Tile-bucketed intersection of C views (``radii [C,N,2]`` ...; ``counts`` filled by ``project_multi``): one scan, one
-    scatter and one sort launch.  View c owns the segment ``[sum(seg[:c]), +seg[c])`` of one keys / vals buffer; offsets
-    [C,T+1] are absolute indices into it and vals = c*N + gaussian (gsplat's concatenated per-camera layout).
+    """Tile-bucketed intersection of C views (``radii [C,N,2]`` ...; ``counts`` filled by ``project_multi``): one scan, the
+    two band-scatter passes and one sort launch.  View c owns the segment ``[sum(seg[:c]), +seg[c])`` of one keys / vals
+    buffer; offsets [C,T+1] are absolute indices into it and vals = c*N + gaussian (gsplat's concatenated per-camera layout).
 
     ``capacities=None``: one host sync reads all C counts and the segments are exactly the counts.  ``capacities`` (C ints):
     no host sync; entries of a view beyond its count are undefined, and a view that needed more is flagged in
@@ -199,8 +211,10 @@ def intersect_multi(radii, splats, tpg, W, H, counts, capacities=None, keys=True
     vals = torch.empty(max(total, 1), dtype=torch.int32, device=dev)
     keys_t = torch.empty(max(total, 1), dtype=torch.int64, device=dev) if keys else None
     packed = torch.empty(max(total, 1), dtype=torch.int64, device=dev)
-    _lib.call("adb_raster_tile_scatter_sort_multi", N, Cn, _lib.ptr(radii), _lib.ptr(splats), _lib.ptr(tpg), W, H, caps,
-              _lib.ptr(counts), _lib.ptr(offsets), _lib.ptr(packed), _lib.ptr(keys_t), _lib.ptr(vals), _lib.stream())
+    scratch = band_scratch(total, dev)
+    _lib.call("adb_raster_tile_band_scatter_sort_multi", N, Cn, _lib.ptr(radii), _lib.ptr(splats), _lib.ptr(tpg), W, H,
+              caps, _lib.ptr(counts), _lib.ptr(offsets), _lib.ptr(packed), _lib.ptr(scratch), scratch.numel(),
+              _lib.ptr(keys_t), _lib.ptr(vals), _lib.stream())
     return (keys_t[:total] if keys else None), vals[:total], offsets, info, seg
 
 
@@ -238,7 +252,7 @@ def blend_backward_multi(W, H, splats, vals, offsets, alphas, last_ids, v_colors
 def intersect(radii, splats, tpg, W, H, cam_id=0, n_cams=1, sort=True, legacy=False, capacity=None, method=None, counts=None):
     """Tile keys/values (sorted), tile offsets [T+1] for one camera.
 
-    ``method="bucket"`` (default): tile-bucketed pipeline — count, scan, scatter, one CTA-local bitonic sort per tile
+    ``method="bucket"`` (default): tile-bucketed pipeline — count, scan, band scatter, one CTA-local bitonic sort per tile
     (csrc/raster_isect.cu) — bit-identical to the stable radix sort of (cam | tile | depth) keys it replaces.
     ``method="radix"`` (or env ADB_ISECT=radix): round-1 path (scan, emit, CUB onesweep radix sort, offsets), kept for A/B.
 
@@ -286,9 +300,10 @@ def intersect(radii, splats, tpg, W, H, cam_id=0, n_cams=1, sort=True, legacy=Fa
         vals = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
         if cap > 0:
             packed = torch.empty(cap, dtype=torch.int64, device=dev)
-            _lib.call("adb_raster_tile_scatter_sort", N, _lib.ptr(radii), _lib.ptr(splats), _lib.ptr(tpg), W, H,
+            scratch = band_scratch(cap, dev)
+            _lib.call("adb_raster_tile_band_scatter_sort", N, _lib.ptr(radii), _lib.ptr(splats), _lib.ptr(tpg), W, H,
                       int(legacy), cam_id, n_cams, cap, _lib.ptr(counts), _lib.ptr(offsets), _lib.ptr(packed),
-                      _lib.ptr(keys), _lib.ptr(vals), _lib.stream())
+                      _lib.ptr(scratch), scratch.numel(), _lib.ptr(keys), _lib.ptr(vals), _lib.stream())
         else:
             counts.zero_()
         if capacity is None:

@@ -185,6 +185,24 @@ int adb_raster_tile_scatter_sort_multi(int N, int C, const int32_t* radii, const
                                        int W, int H, const long long* capacities /*HOST [C]*/, int32_t* tile_counts,
                                        const int32_t* tile_offsets, void* packed, int64_t* keys, int32_t* vals,
                                        adb_stream_t stream);
+/* Band scatter: the same results as adb_raster_tile_scatter_sort(_multi), bit for bit, with the scatter's writes in runs.
+ *   band pass  one (Gaussian, tile row) pair per tile row a splat touches, appended per CTA in runs to the row's region
+ *              of `scratch` (the row's tile segments; pairs of a row cut by the capacity are rebuilt from the splats);
+ *   tile pass  one CTA per (tile row, view) expands the row's pairs into its tiles' segments of `packed`;
+ *   sort       as adb_raster_tile_scatter_sort.
+ * scratch: adb_raster_tile_band_scratch_bytes(sum of the capacities) bytes, no initialisation.  tile_counts as left by the
+ * scan (the first half returns to zero); its per-tile segment starts are used, and overwritten, as per-row cursors.
+ * W and H at most 65536 (4096 tiles). */
+int adb_raster_tile_band_scratch_bytes(long long capacity, size_t* bytes);
+int adb_raster_tile_band_scatter_sort(int N, const int32_t* radii, const float* splats, const int32_t* tiles_per_gauss, int W,
+                                      int H, int legacy, int cam_id, int n_cams, long long capacity, int32_t* tile_counts,
+                                      const int32_t* tile_offsets, void* packed, void* scratch, size_t scratch_bytes,
+                                      int64_t* keys, int32_t* vals, adb_stream_t stream);
+int adb_raster_tile_band_scatter_sort_multi(int N, int C, const int32_t* radii, const float* splats,
+                                            const int32_t* tiles_per_gauss, int W, int H,
+                                            const long long* capacities /*HOST [C]*/, int32_t* tile_counts,
+                                            const int32_t* tile_offsets, void* packed, void* scratch, size_t scratch_bytes,
+                                            int64_t* keys, int32_t* vals, adb_stream_t stream);
 int adb_raster_blend_fwd(int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
                          const int32_t* tile_offsets, float* colors /*[H,W,4]*/, float* alphas /*[H,W]*/,
                          int32_t* last_ids /*[H,W]*/, adb_stream_t stream);
