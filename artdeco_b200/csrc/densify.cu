@@ -13,6 +13,7 @@
 // Arithmetic follows what PyTorch evaluates on CUDA: a division by a Python scalar is a multiplication by the fp32
 // reciprocal, and the steps the reference runs as separate kernels are rounded separately here (__fmul_rn / __fadd_rn).
 #include "common.cuh"
+#include "resample.cuh"
 #include "select.cuh"
 #include "artdeco_b200.h"
 
@@ -20,6 +21,9 @@
 
 namespace {
 
+using adb_resample::blend4;
+using adb_resample::lin_src;
+using adb_resample::pool4;
 using adb_select::HIST_BINS;
 using adb_select::SEL_THREADS;
 
@@ -54,28 +58,10 @@ __device__ __forceinline__ float clampf(float x, float lo, float hi) {        //
     return x != x ? x : fminf(fmaxf(x, lo), hi);
 }
 
-// upsample_bilinear2d (align_corners=True) source index: (index, neighbour offset, lambda)
-__device__ __forceinline__ void lin_src(float scale, int dst, int in_size, int* i0, int* ip, float* l1) {
-    const float r = scale * (float)dst;
-    const int i = (int)r;
-    *i0 = i;
-    *ip = (i < in_size - 1) ? 1 : 0;
-    *l1 = r - (float)i;
-}
-
 // avg_pool2d(image, 2) at pooled pixel (py, px) of channel c
 __device__ __forceinline__ float pooled(const float* __restrict__ img, int W, size_t plane, int c, int py, int px) {
     const float* p = img + c * plane + (size_t)(2 * py) * W + 2 * px;
-    float a = 0.f;
-    a = __fadd_rn(a, p[0]);
-    a = __fadd_rn(a, p[1]);
-    a = __fadd_rn(a, p[W]);
-    a = __fadd_rn(a, p[W + 1]);
-    return a / 4.0f;
-}
-
-__device__ __forceinline__ float blend4(float h0l, float h1l, float w0l, float w1l, float a, float b, float c, float d) {
-    return h0l * (w0l * a + w1l * b) + h1l * (w0l * c + w1l * d);
+    return pool4(p[0], p[1], p[W], p[W + 1]);
 }
 
 // img = interpolate(avg_pool2d(image, 2), (h, w), bilinear, align_corners=True)  at LoD pixel (y, x), 3 channels

@@ -21,6 +21,7 @@
 #include <cfloat>
 
 #include "common.cuh"
+#include "mapper_pose.cuh"
 #include "sim3.cuh"
 
 namespace {
@@ -29,34 +30,8 @@ constexpr int NT_FRAMES = 128;
 constexpr int NT_ROWS = 256;
 constexpr int DELTA_FLOATS = 16;   // rows 0..2 of the 4x4 delta, then [12] = 1 if the frame has a delta, 0 if singular
 
-// sixD2mtx (Reconstruct/utils.py:223-229) of r [3,2] row-major: columns b1, b2, b3 = b1 x b2.
-__device__ __forceinline__ void six_d_to_R(const float* r, float R[3][3]) {
-    float b1[3] = {r[0], r[2], r[4]};
-    const float c[3] = {r[1], r[3], r[5]};
-    const float n1 = sqrtf(b1[0] * b1[0] + b1[1] * b1[1] + b1[2] * b1[2]);
-#pragma unroll
-    for (int i = 0; i < 3; ++i) b1[i] = b1[i] / n1;
-    const float d = b1[0] * c[0] + b1[1] * c[1] + b1[2] * c[2];
-    float b2[3];
-#pragma unroll
-    for (int i = 0; i < 3; ++i) b2[i] = c[i] - d * b1[i];
-    const float n2 = sqrtf(b2[0] * b2[0] + b2[1] * b2[1] + b2[2] * b2[2]);
-#pragma unroll
-    for (int i = 0; i < 3; ++i) b2[i] = b2[i] / n2;
-    const float b3[3] = {b1[1] * b2[2] - b1[2] * b2[1], b1[2] * b2[0] - b1[0] * b2[2], b1[0] * b2[1] - b1[1] * b2[0]};
-#pragma unroll
-    for (int i = 0; i < 3; ++i) {
-        R[i][0] = b1[i];
-        R[i][1] = b2[i];
-        R[i][2] = b3[i];
-    }
-}
-
-// c = -R^T t
-__device__ __forceinline__ void centre_of(const float R[3][3], const float t[3], float c[3]) {
-#pragma unroll
-    for (int j = 0; j < 3; ++j) c[j] = -(R[0][j] * t[0] + R[1][j] * t[1] + R[2][j] * t[2]);
-}
+using adb_pose::centre_of;
+using adb_pose::six_d_to_R;
 
 // out [4,4] = inverse of [R | t; 0 0 0 1] = [R^T | -R^T t; 0 0 0 1]
 __device__ __forceinline__ void store_rigid_inverse(const float R[3][3], const float t[3], float* out) {
@@ -70,13 +45,6 @@ __device__ __forceinline__ void store_rigid_inverse(const float R[3][3], const f
         out[4 * i + 3] = c[i];
     }
     out[12] = 0.f; out[13] = 0.f; out[14] = 0.f; out[15] = 1.f;
-}
-
-// pypose's quat2unit: q / max(|q|, 1e-12)
-__device__ __forceinline__ void quat_unit(float q[4]) {
-    const float n = fmaxf(sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]), 1e-12f);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) q[i] = q[i] / n;
 }
 
 __global__ void __launch_bounds__(NT_FRAMES)
@@ -122,20 +90,10 @@ reanchor_keyframes_kernel(int K, int K_slam, const float* __restrict__ slam_T_WC
         for (int i = 0; i < 3; ++i) t[i] = y[i] * A[7] + A[i];
         adb_sim3::quat_comp(qa, qb, q);
     }
-    quat_unit(q);
-    // new_Rt = T_WCf.Inv().matrix(): q^-1 = conj(q), t^-1 = -(q^-1 t), columns of R = q^-1 e_c
-    const float qi[4] = {-q[0], -q[1], -q[2], q[3]};
-    float ti[3];
-    adb_sim3::act_so3(qi, t, ti);
-    ti[0] = -ti[0]; ti[1] = -ti[1]; ti[2] = -ti[2];
-    float R_new[3][3];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-        const float e[3] = {c == 0 ? 1.f : 0.f, c == 1 ? 1.f : 0.f, c == 2 ? 1.f : 0.f};
-        float col[3];
-        adb_sim3::act_so3(qi, e, col);
-        R_new[0][c] = col[0]; R_new[1][c] = col[1]; R_new[2][c] = col[2];
-    }
+    adb_pose::quat_unit(q);
+    // new_Rt = T_WCf.Inv().matrix()
+    float ti[3], R_new[3][3];
+    adb_pose::se3_inverse_Rt(t, q, R_new, ti);
     store_rigid_inverse(R_new, ti, new_c2w + 16 * (size_t)k);               // torch.linalg.inv(new_Rt)
     // set_Rt(new_Rt)
 #pragma unroll

@@ -95,6 +95,38 @@ int adb_reanchor_gaussians(long long N, int K, const long long* ids, const float
                            const float* old_c2w, const float* new_c2w, float* xyz_out, float* rotation_out, int32_t* n_bad,
                            void* ws, size_t ws_bytes, adb_stream_t stream);
 
+/* ---- key-frame hand-off from the Backend to the mapper (csrc/keyframe.cu) ----
+ *   adb_kf_dense_point      replaces Backend.prepare_for_mapper / compute_dense_point (VSLAM/Backend.py:117-193) at SLAM
+ *                           resolution H x W.  X_canon [HW,3], K [3,3] row-major, dense_point [HW,4] (16-byte aligned).
+ *                           last_T_WC == NULL is the first key frame: points = constrain_points_to_ray(X_canon), channel 3 =
+ *                           float(C[p] * fp32(1 / N) > 1.5) with C [HW] and N a device int32 [1]; nothing else is read or
+ *                           written.  Otherwise, with T_WC / last_T_WC the Sim(3) poses (tx ty tz qx qy qz qw s) of the key
+ *                           frame and of the last key frame and idx_k2l [HW] int64: points = SE3(T_WC[:7]).Inv().Act(
+ *                           T_WC.Act(Xc)) in key-frame pixel order, channel 3 = the reprojection confidence of
+ *                           Xc[idx_k2l[p]] in the last key frame at its pixel p (1 below 3 px, else 1 / (r - 2)), and
+ *                           T_CkC [8] = last_T_WC^-1 T_WC.  A pixel whose idx_k2l is outside [0, HW) is NaN in all four
+ *                           channels and adds 1 to *n_bad (device int32, caller-zeroed).  One launch.
+ *   adb_kf_pyramid_floats   floats of the packed pyramids of an H x W mapper image with pyr_levels levels (sizes floored
+ *                           level by level): idepth_floats = sum of h_l w_l over levels 0.., image_floats = 3 h_l w_l over
+ *                           levels 1.. (level 0 of the image pyramid is the image itself).
+ *   adb_kf_mapper_inputs    replaces run_system.py:164-192 and Keyframe.__init__'s training branch
+ *                           (Reconstruct/scene/keyframe.py:64-127) for an H x W mapper image, 1 <= pyr_levels <= 6.
+ *                           image [3,H,W] read through image_strides (HOST [3], elements: channel, row, column);
+ *                           dense_point [Hs,Ws,4] as adb_kf_dense_point writes it.  idepth_pyr: levels 0.. packed, level 0 =
+ *                           interpolate(where(z != 0, 1 / (z + 1e-4), 1e4), (H, W), bilinear, align_corners=True), level l =
+ *                           avg_pool2d(level l-1, 2); image_pyr: levels 1.. packed, [3,h_l,w_l] each (NULL if pyr_levels
+ *                           == 1).  From Rt = quat2unit(SE3(T_WC[:7])).Inv().matrix(): rW2C [3,2] = Rt[:3,:2], tW2C [3] =
+ *                           Rt[:3,3], approx_centre [3] = -Rt[:3,:3]^T Rt[:3,3] and R [3,3] = sixD2mtx(rW2C).  One launch. */
+int adb_kf_dense_point(int height, int width, const float* X_canon, const float* C, const int32_t* N, const float* T_WC,
+                       const float* last_T_WC, const long long* idx_k2l, const float* K, float* dense_point, float* T_CkC,
+                       int32_t* n_bad, adb_stream_t stream);
+int adb_kf_pyramid_floats(int height, int width, int pyr_levels, long long* idepth_floats /*HOST*/,
+                          long long* image_floats /*HOST*/);
+int adb_kf_mapper_inputs(int height, int width, int Hs, int Ws, int pyr_levels, const float* image,
+                         const long long* image_strides /*HOST [3]*/, const float* dense_point, const float* T_WC,
+                         float* idepth_pyr, float* image_pyr, float* rW2C, float* tW2C, float* approx_centre, float* R,
+                         adb_stream_t stream);
+
 /* ---- Gaussian-splat rasterizer (one camera per call) ----
  * replaces the stages of gsplat.rendering.rasterization as called at
  * Reconstruct/scene/scene_models/h3dgsv3.py:664-680 (gsplat itself is an un-vendored pip dependency).
