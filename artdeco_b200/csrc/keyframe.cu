@@ -21,11 +21,14 @@
 //    avg_pool2d's window-order sum (resample.cuh).
 #include <cstdint>
 
+#include "backproject.cuh"
 #include "common.cuh"
 #include "mapper_pose.cuh"
 #include "resample.cuh"
 
 namespace {
+
+using adb_backproject::on_ray;
 
 constexpr int DP_THREADS = 256;
 constexpr int TILE = 32;               // mapper tile edge at level 0
@@ -79,15 +82,6 @@ __device__ __forceinline__ void sim3_mul(const float* A, const float* B, float* 
     T[5] = __fadd_rn(__fsub_rn(__fadd_rn(__fmul_rn(a[3], b[2]), __fmul_rn(a[0], b[1])), __fmul_rn(a[1], b[0])), __fmul_rn(a[2], b[3]));
     T[6] = __fsub_rn(__fsub_rn(__fsub_rn(__fmul_rn(a[3], b[3]), __fmul_rn(a[0], b[0])), __fmul_rn(a[1], b[1])), __fmul_rn(a[2], b[2]));
     T[7] = __fmul_rn(A[7], B[7]);
-}
-
-// constrain_points_to_ray of pixel p: z (ray through the pixel), K row-major [3,3]
-__device__ __forceinline__ void on_ray(const float* __restrict__ X, const float* k, int p, int W, float P[3]) {
-    const float z = __ldg(X + 3 * (size_t)p + 2);
-    const float u = (float)(p % W), v = (float)(p / W);
-    P[0] = __fmul_rn(z, __fdiv_rn(__fsub_rn(u, k[2]), k[0]));
-    P[1] = __fmul_rn(z, __fdiv_rn(__fsub_rn(v, k[5]), k[4]));
-    P[2] = z;
 }
 
 __global__ void __launch_bounds__(DP_THREADS)

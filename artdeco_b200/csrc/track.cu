@@ -11,6 +11,7 @@
 //   track_step        one CTA: CTA partials summed in fp64 in a fixed order, 7x7 Cholesky in fp64, Exp(tau) T, quat2unit,
 //                     check_convergence.
 // Every sum has a fixed order and the histograms count integers, so results are bitwise reproducible run to run.
+#include "backproject.cuh"
 #include "common.cuh"
 #include "select.cuh"
 #include "sim3.cuh"
@@ -85,8 +86,9 @@ track_cov_kernel(int H, int W, const float* __restrict__ Kd, const float* __rest
         gx = gx < 0 ? -gx : (gx >= W ? 2 * W - 2 - gx : gx);
         gy = min(max(gy, 0), H - 1);           // rows / columns past a partial tile feed no output
         gx = min(max(gx, 0), W - 1);
-        const float z = Xff[((size_t)gy * W + gx) * 3 + 2];
-        const float x = ((float)gx - cx) / fx * z, y = ((float)gy - cy) / fy * z;
+        float P[3];
+        adb_backproject::ray_point((float)gx, (float)gy, Xff[((size_t)gy * W + gx) * 3 + 2], fx, fy, cx, cy, P);
+        const float x = P[0], y = P[1], z = P[2];
         const float v = (isfinite(x) && isfinite(y) && isfinite(z) && z > 0.f) ? 1.f : 0.f;
         sm[0][sy][sx] = v;
         sm[1][sy][sx] = x * v; sm[2][sy][sx] = y * v; sm[3][sy][sx] = z * v;
@@ -137,10 +139,10 @@ track_gather_kernel(PrepParams p, const float* __restrict__ Kd, const long long*
         jl = jl < 0 ? 0 : (jl >= p.n ? p.n - 1 : jl);    // memory safety only: matching emits indices in [0, N)
         const int j = (int)jl;
         const int uj = j % p.W, vj = j / p.W, ui = i % p.W, vi = i / p.W;
-        const float z = Xff[(size_t)j * 3 + 2];
-        Xf[(size_t)i * 3 + 0] = ((float)uj - cx) / fx * z;
-        Xf[(size_t)i * 3 + 1] = ((float)vj - cy) / fy * z;
-        Xf[(size_t)i * 3 + 2] = z;
+        float P[3];
+        adb_backproject::ray_point((float)uj, (float)vj, Xff[(size_t)j * 3 + 2], fx, fy, cx, cy, P);
+#pragma unroll
+        for (int d = 0; d < 3; ++d) Xf[(size_t)i * 3 + d] = P[d];
 #pragma unroll
         for (int d = 0; d < 3; ++d) Xf_cov[(size_t)i * 3 + d] = cov_f[(size_t)j * 3 + d];
         const float q = sqrtf(Qff[j] * Qkf[i]);

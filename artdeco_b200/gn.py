@@ -28,27 +28,44 @@ def _solve(mode, Twc, Xs, Cs, K, ii, jj, idx_ii2jj, valid_match, Q, height, widt
     upper triangle still holds the assembled matrix, the lower triangle and the diagonal hold the Cholesky factor), b [D]
     f64 (the solution x, dx = -x), S [E,28] f32 (lower triangle, row-major) and v [E,7] f32; D = 7 (K-1)."""
     _lib.require_cuda(Twc)
+    if jj.shape[0] != ii.shape[0]:
+        raise ValueError("ii and jj must list the same edges")
+    # gn_kernels.cu:160-171: unique sorted key-frame ids; edges address the pose table by their rank in it
+    unique = torch.unique(torch.cat([ii, jj]), sorted=True)
+    if unique.numel() > int(Xs.shape[0]):
+        # a rank >= K would address a pose (and a pointmap) past the end of the tables
+        raise ValueError(f"the edges name {unique.numel()} key frames but Twc has {int(Xs.shape[0])} rows")
+    ii_pos = torch.searchsorted(unique, ii.contiguous()).long().contiguous()
+    jj_pos = torch.searchsorted(unique, jj.contiguous()).long().contiguous()
+    return solve_positions(mode, Twc, Xs, Cs, K, ii_pos, jj_pos, idx_ii2jj, valid_match, Q, height, width, pixel_border,
+                           z_eps, sigma_a, sigma_b, C_thresh, Q_thresh, max_iter, delta_thresh, return_state,
+                           return_workspace)
+
+
+def solve_positions(mode, Twc, Xs, Cs, K, ii_pos, jj_pos, idx_ii2jj, valid_match, Q, height, width, pixel_border, z_eps,
+                    sigma_a, sigma_b, C_thresh, Q_thresh, max_iter, delta_thresh, return_state=False,
+                    return_workspace=False):
+    """The solve with the edges given as positions in the pose table (int64 [E], each in ``[0, K)``, the caller's to
+    guarantee): no ``unique`` and nothing that reads the device from the host, so a caller that keeps its edge list on
+    the host (``factor_graph.FactorGraph``) runs the whole solve without a sync.  Same arguments and results as ``_solve``
+    otherwise."""
+    _lib.require_cuda(Twc)
     dev = Twc.device
     if Twc.dim() != 2 or Twc.shape[1] != 8 or Twc.dtype != torch.float32:
         raise ValueError("Twc must be a float32 [K,8] tensor (t, q xyzw, s)")
     Kp, n = int(Xs.shape[0]), int(Xs.shape[1])
     if Twc.shape[0] != Kp or Cs.shape[0] != Kp:
         raise ValueError("Twc, Xs and Cs must stack the same key frames")
-    E = int(ii.shape[0])
-    if jj.shape[0] != E:
+    E = int(ii_pos.shape[0])
+    if jj_pos.shape[0] != E:
         raise ValueError("ii and jj must list the same edges")
     for name, t in (("idx_ii2jj", idx_ii2jj), ("valid_match", valid_match), ("Q", Q)):
         if t.numel() != E * n:
             raise ValueError(f"{name} must hold E*n = {E * n} elements, got {t.numel()}")
     if mode == 1 and n != int(height) * int(width):
         raise ValueError(f"calib mode needs one point per pixel: n = {n} but height*width = {int(height) * int(width)}")
-    # gn_kernels.cu:160-171: unique sorted key-frame ids; edges address the pose table by their rank in it
-    unique = torch.unique(torch.cat([ii, jj]), sorted=True)
-    if unique.numel() > Kp:
-        # a rank >= K would address a pose (and a pointmap) past the end of the tables
-        raise ValueError(f"the edges name {unique.numel()} key frames but Twc has {Kp} rows")
-    ii_pos = torch.searchsorted(unique, ii.contiguous()).long().contiguous()
-    jj_pos = torch.searchsorted(unique, jj.contiguous()).long().contiguous()
+    ii_pos = ii_pos.long().contiguous()
+    jj_pos = jj_pos.long().contiguous()
     poses = Twc if Twc.is_contiguous() else Twc.contiguous()
     Xc = Xs.detach().float().contiguous()
     Cc = Cs.detach().float().reshape(Kp, n).contiguous()

@@ -373,6 +373,49 @@ int adb_gauss_newton(int mode, int n_poses, int n_pts, int n_edges, float* poses
                      const unsigned char* valid_match, const float* Q, int height, int width, int pixel_border, float z_eps,
                      float sigma_a, float sigma_b, float C_thresh, float Q_thresh, int max_iter, float delta_thresh,
                      float* dx_out, int* state_out, void* ws, size_t ws_bytes, adb_stream_t stream);
+/* ---- the Backend's factor graph around the global solve (csrc/factor_graph.cu) ----
+ * replaces FactorGraph (VSLAM/mast3r_slam/global_opt.py) except the solve, which is adb_gauss_newton.  Two-way edge table
+ * of n pixels per row, caller-owned, `capacity` edges = 2 capacity rows: rows_i / rows_j int64 [2 capacity],
+ * rows_idx int64 [2 capacity, n], rows_valid uint8 [2 capacity, n], rows_Q [2 capacity, n].  Edge e is row 2e =
+ * (i, j, idx_i2j, valid_match_j, Qj) and row 2e+1 = (j, i, idx_j2i, valid_match_i, Qi), the matcher's masks as the
+ * reference stores them (the solve applies Q_conf itself): the first 2E rows are adb_gauss_newton's
+ * ii / jj (once mapped to pose positions), idx_ii2jj, valid_match and Q.
+ *   adb_fg_gate               add_factors after matching (:56-110) for B <= 1024 candidate edges.  cand_ij int64 [B,2]
+ *                             (i, j); idx_i2j / idx_j2i int64 [B,n]; valid_match_j / _i uint8 [B,n]; Qii, Qjj, Qji, Qij
+ *                             [B,n].  Per pixel Qj = sqrt(Qii[b, idx_i2j] Qji), valid_j = valid_match_j & (Qj > Q_conf),
+ *                             and the same for i.  Per edge the valid counts are summed in integers, match_frac =
+ *                             count * fp32(1 / n), and the edge is invalid when min(frac_j, frac_i) < min_match_frac
+ *                             unless i == j - 1; with is_reloc one invalid edge rejects all B.  Accepted edges are written
+ *                             in candidate order at edges n_edges.. of the table (capacity >= n_edges + B: rows up to edge
+ *                             n_edges + B - 1 are used as scratch).  accepted int32 [B] (0/1), counts int32 [B,2] (valid_j,
+ *                             valid_i).  An index outside [0, n) is not read: its pixel is an invalid match with Q = NaN,
+ *                             and it adds 1 to *n_bad (device int32, accumulated).  ws from adb_fg_gate_workspace_bytes.
+ *                             Three launches (two when B == 1).
+ *   adb_fg_mirror_refresh     the solve's key-frame inputs (get_poses_points, constrain_points_to_ray; :120-126,187-188):
+ *                             for each of `rows` rows, mirror row d = ids ? ids[r] : r (rows with d outside
+ *                             [0, mirror_rows) are skipped) gets Xm [d] = X (mode 0, rays) or constrain_points_to_ray(X)
+ *                             with K [3,3] (mode 1, calib) and Cm [d] = C * fp32(1 / N).  The source row is r when `staged`
+ *                             (X [rows,n,3], C [rows,n], N [rows] copied by the caller) and d otherwise (the key-frame store's
+ *                             own stacked tensors).  With seen != NULL (int32 [mirror_rows,2]), a row whose (dataset_idx,
+ *                             N_updates) equals seen[d] is left as it is, and every row's current pair is written to
+ *                             seen_next[d] (another buffer: the caller alternates them).  One launch.
+ *   adb_fg_pose_gather        poses [U,8] = quat2unit(T_WC[ids ? ids[r] : r]) for r < U; T_WC [src_rows,8].  One launch.
+ *   adb_fg_pose_scatter       update_T_WCs(T_WCs[pin:], unique[pin:]): T_WC[ids ? ids[r] : r] = poses[r] for pin <= r < U;
+ *                             nothing when U <= pin.  One launch. */
+int adb_fg_gate_workspace_bytes(int B, int n, size_t* bytes /*HOST*/);
+int adb_fg_gate(int B, int n, long long n_edges, long long capacity, const long long* cand_ij, const long long* idx_i2j,
+                const long long* idx_j2i, const unsigned char* valid_match_j, const unsigned char* valid_match_i,
+                const float* Qii, const float* Qjj, const float* Qji, const float* Qij, float Q_conf, float min_match_frac,
+                int is_reloc, long long* rows_i, long long* rows_j, long long* rows_idx, unsigned char* rows_valid,
+                float* rows_Q, int* accepted, int* counts, int* n_bad, void* ws, size_t ws_bytes, adb_stream_t stream);
+int adb_fg_mirror_refresh(int mode, int rows, int height, int width, int mirror_rows, const long long* ids, int staged,
+                          const float* X, const float* C, const int32_t* N, const int32_t* dataset_idx,
+                          const int32_t* N_updates, const int32_t* seen, int32_t* seen_next, const float* K, float* Xm,
+                          float* Cm, adb_stream_t stream);
+int adb_fg_pose_gather(int n_unique, int src_rows, const long long* ids, const float* T_WC, float* poses,
+                       adb_stream_t stream);
+int adb_fg_pose_scatter(int n_unique, int pin, int dst_rows, const long long* ids, const float* poses, float* T_WC,
+                        adb_stream_t stream);
 /* Frame tracking: CameraTracker.track after matching (VSLAM/CameraTracker.py:53-155), calibrated Sim(3) only
  * (optimize_focal is not supported).  N = height * width points in KEY-FRAME pixel order; poses [8] = (t, q xyzw, s).
  * Three calls on one stream share `ws` and the device `state` block; none synchronises the host:
