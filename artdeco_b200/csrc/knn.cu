@@ -8,8 +8,23 @@
 // with a scalar, uncoalesced gather (points[indices[i]]), after two blocking D2H copies of the bounding box.
 // Here: bounding box, grid sizing and cell ids stay on the device; points are radix-sorted by cell id and
 // REORDERED into a float4 array (x,y,z,original index), so a row of x-adjacent cells is one contiguous,
-// coalesced bucket scan; each query searches Chebyshev shells r = 0,1,2,.. and stops as soon as the K-th best
-// distance is <= (r*h)^2, which makes the result exact.
+// coalesced bucket scan; each query searches Chebyshev shells r = 0,1,2,.. of cells.
+//
+// Exactness.  A point's cell is floor(fl(fl(x - minx) * fl(1/h))): three roundings, so the computed coordinate
+// (in cells) is within 3*2^-24 * n of the true (x - minx)/h, n = the largest cell count of any axis (clamping
+// into [0, n-1] only moves a point further from the cells it is clamped away from).  Two points whose cells
+// differ by r+1 along an axis are therefore more than (r - slack)*h apart, slack = 2 * 8*2^-24 * n = n*2^-20
+// (8 ulps per coordinate, with margin).  The search stops after shell r once the K-th best squared distance is
+// <= ((0.99999*r - slack)*h)^2; the factor 0.99999 covers the relative rounding of the fp32 distance (a few
+// ulps) and of the bound itself.  Every point not yet visited is then no closer than the K-th best, and the
+// result equals the brute force.  On wide grids (hundreds of cells per axis) the fixed 0.99999 alone is not
+// enough: a point two cells away can be up to ~4e-5 of a cell closer than 1*h.
+// Points with a NaN, an infinite or a coordinate above kFar in magnitude are nobody's neighbour: their squared
+// distance to any point near the rest of the cloud overflows fp32, which the brute force never selects.  They
+// are left out of the bounding box (one such point would otherwise stretch the grid until every other point
+// shares a cell), get a key past the last cell, so they sort to the end and are never scanned, and their own
+// row is FLT_MAX / -1 (distCUDA2: inf).  The one difference from the brute force: two such points closer than
+// sqrt(FLT_MAX) to each other are not each other's neighbours here.
 // Squared distances are evaluated as fma(dz,dz,fma(dx,dx,dy*dy)) — the contraction nvcc applies to the
 // reference's `d.x*d.x + d.y*d.y + d.z*d.z` (simple_knn.cu:136,400) — so distCUDA2 is bit-reproducible.
 #include "common.cuh"
@@ -21,7 +36,15 @@ namespace {
 struct Grid {
     float minx, miny, minz, h, inv_h;
     int nx, ny, nz, ncells;
+    float slack;  // worst-case error of a cell coordinate difference, in cells (see the header)
 };
+
+// |coordinate| above this makes a point unusable (its squared distance to the origin exceeds FLT_MAX)
+constexpr float kFar = 1.8e19f;
+
+__device__ __forceinline__ bool usable(float x, float y, float z) {
+    return fabsf(x) <= kFar && fabsf(y) <= kFar && fabsf(z) <= kFar;  // false for NaN and +-inf too
+}
 
 struct Ws {  // carved out of the caller's workspace
     Grid* grid;
@@ -73,13 +96,15 @@ __global__ void bbox_init_kernel(unsigned* bbox) {
 __global__ void __launch_bounds__(256)
 bbox_kernel(long long P, const float* __restrict__ pts, unsigned* __restrict__ bbox) {
     float mn[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, mx[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < P; i += (long long)gridDim.x * blockDim.x)
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < P; i += (long long)gridDim.x * blockDim.x) {
+        const float v[3] = {pts[3 * i], pts[3 * i + 1], pts[3 * i + 2]};
+        if (!usable(v[0], v[1], v[2])) continue;
 #pragma unroll
         for (int a = 0; a < 3; ++a) {
-            float v = pts[3 * i + a];
-            mn[a] = fminf(mn[a], v);
-            mx[a] = fmaxf(mx[a], v);
+            mn[a] = fminf(mn[a], v[a]);
+            mx[a] = fmaxf(mx[a], v[a]);
         }
+    }
 #pragma unroll
     for (int a = 0; a < 3; ++a)
 #pragma unroll
@@ -95,19 +120,23 @@ bbox_kernel(long long P, const float* __restrict__ pts, unsigned* __restrict__ b
         }
 }
 
-// single thread: choose the cell size so that a cell holds ~4 points, with at most 2P+64 cells
+// single thread: choose the cell size so that a cell holds ~4 points, with at most 2P+64 cells.  The volume is
+// formed in double: extents up to 2*kFar would overflow fp32.  With no usable point the box is empty (min > max)
+// and the grid is one cell at the origin.
 __global__ void grid_setup_kernel(long long P, const unsigned* bbox, Grid* g) {
     float mn[3], e[3];
     float emax = 0.f;
     for (int a = 0; a < 3; ++a) {
-        mn[a] = o2f(bbox[a]);
-        e[a] = fmaxf(o2f(bbox[3 + a]) - mn[a], 0.f);
+        const float lo = o2f(bbox[a]), hi = o2f(bbox[3 + a]);
+        const bool empty = !(lo <= hi);
+        mn[a] = empty ? 0.f : lo;
+        e[a] = empty ? 0.f : hi - lo;
         emax = fmaxf(emax, e[a]);
     }
     if (!(emax > 0.f)) emax = 1.f;
-    float vol = 1.f;
-    for (int a = 0; a < 3; ++a) vol *= fmaxf(e[a], 1e-3f * emax);
-    float h = cbrtf(4.0f * vol / (float)P);
+    double vol = 1.0;
+    for (int a = 0; a < 3; ++a) vol *= (double)fmaxf(e[a], 1e-3f * emax);
+    float h = (float)cbrt(4.0 * vol / (double)P);
     if (!(h > 0.f)) h = emax;
     const long long cap = 2 * P + 64;
     int n[3];
@@ -125,6 +154,7 @@ __global__ void grid_setup_kernel(long long P, const unsigned* bbox, Grid* g) {
     g->h = h; g->inv_h = 1.0f / h;
     g->nx = n[0]; g->ny = n[1]; g->nz = n[2];
     g->ncells = n[0] * n[1] * n[2];
+    g->slack = (float)max(n[0], max(n[1], n[2])) * 0x1p-20f;
 }
 
 __device__ __forceinline__ void cell_of(const Grid& g, float x, float y, float z, int& cx, int& cy, int& cz) {
@@ -139,9 +169,10 @@ cell_id_kernel(long long P, const float* __restrict__ pts, const Grid* __restric
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P) return;
     const Grid g = *gp;
+    const float x = pts[3 * i], y = pts[3 * i + 1], z = pts[3 * i + 2];
     int cx, cy, cz;
-    cell_of(g, pts[3 * i], pts[3 * i + 1], pts[3 * i + 2], cx, cy, cz);
-    keys[i] = (unsigned)((cz * g.ny + cy) * g.nx + cx);
+    cell_of(g, x, y, z, cx, cy, cz);
+    keys[i] = usable(x, y, z) ? (unsigned)((cz * g.ny + cy) * g.nx + cx) : (unsigned)g.ncells;  // past the last cell
     vals[i] = (int)i;
 }
 
@@ -205,7 +236,8 @@ knn_query_kernel(long long P, long long Q, int K, const Grid* __restrict__ gp, c
     cell_of(g, me.x, me.y, me.z, cx, cy, cz);
     Best<KMAX> best;
     best.init();
-    const int rmax = max(g.nx, max(g.ny, g.nz));
+    // an unusable query keeps the empty row
+    const int rmax = usable(me.x, me.y, me.z) ? max(g.nx, max(g.ny, g.nz)) : -1;
     for (int r = 0; r <= rmax; ++r) {
         const int z0 = max(cz - r, 0), z1 = min(cz + r, g.nz - 1);
         const int y0 = max(cy - r, 0), y1 = min(cy + r, g.ny - 1);
@@ -235,9 +267,9 @@ knn_query_kernel(long long P, long long Q, int K, const Grid* __restrict__ gp, c
                     }
                 }
             }
-        // everything not yet visited is at least r*h away
+        // everything not yet visited is more than (r - slack)*h away (see the header)
         const int kth = (MODE == 0 ? 3 : K) - 1;
-        const float bound = (float)r * g.h * 0.99999f;
+        const float bound = fmaxf((float)r * 0.99999f - g.slack, 0.f) * g.h;
         float kth_d = FLT_MAX;
 #pragma unroll
         for (int k = 0; k < KMAX; ++k)
@@ -263,8 +295,8 @@ int build_grid(long long P, const float* points, const Ws& w, cudaStream_t strea
     grid_setup_kernel<<<1, 1, 0, stream>>>(P, w.bbox, w.grid);
     cell_id_kernel<<<adb_cdiv(P, 256), 256, 0, stream>>>(P, points, w.grid, w.keys_a, w.vals_a);
     ADB_CHECK_LAUNCH("knn grid kernels");
-    int bits = 1;
-    while (((long long)1 << bits) < 2 * P + 64) ++bits;
+    int bits = 1;  // keys go up to ncells <= 2P+64 (the unusable points' key)
+    while (((long long)1 << bits) <= 2 * P + 64) ++bits;
     cub::DoubleBuffer<unsigned> dk(w.keys_a, w.keys_b);
     cub::DoubleBuffer<int> dv(w.vals_a, w.vals_b);
     size_t need = w.cub_bytes;
