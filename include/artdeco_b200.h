@@ -69,6 +69,47 @@ int adb_mapper_loss_backward(int height, int width, const float* colors, const f
                              float* v_colors, float* v_alphas, float* v_exposure, void* ws, size_t ws_bytes,
                              adb_stream_t stream);
 
+/* ---- held-out key-frame evaluation (csrc/evaluate.cu) ----
+ * replaces SceneModel.harmonize_test_exposure, Reconstruct/scene/scene_models/h3dgsv3.py:507-520, and the metric loop of
+ * SceneModel.evaluate (:523-558) with psnr (Reconstruct/utils.py:86-87), fused_ssim(train=False) and
+ * lpips.LPIPS(net="vgg") (:98; version 0.1, lpips=True, spatial=False, normalize=False).
+ *   adb_eval_harmonize       exposure [K,3,4] IN PLACE, is_test [K] uint8: the reference loop in order (a test frame after a
+ *                            test frame averages the updated one; idxm = 1 at index 0, idxp = K - 2 at the last index,
+ *                            negative indices wrap as Python's do).  An index outside [-K, K) raises IndexError in the
+ *                            reference: the loop stops there and *n_bad (device int) = 1, else 0
+ * T views of h x w share one evaluation workspace (adb_eval_workspace_bytes; n_gaussians the length of the visibility mask):
+ *   adb_eval_count_visible   view t's visibility_filter [n] (uint8) -> per-CTA counts (replaces .sum().item())
+ *   adb_eval_image_metrics   colors [T,h,w,4] (16-byte aligned) / alphas [T,h,w] the rasterizer's raw outputs; view t uses
+ *                            exposure row view_frame[t] (int32) of the [K,3,4] table.  image [T,3,h,w] = clamp(E[:, :3] rgb +
+ *                            E[:, 3], 0, 1) (render_from_id with bg = 0); gt [T,3,h,w]; ssim_map [T,3,h,w] scratch.
+ *                            Writes per-CTA partials of the squared error and of the SSIM map (adb_ssim_forward, B = T)
+ *   adb_lpips_vgg_forward    frames [frame0, frame0 + n_frames) of img0 = image and img1 = gt, both [T,3,h,w] (h, w >= 16),
+ *                            through VGG16 to relu5_3 as a batch of 2 n_frames.  w1 [64,3,3,3] / b1 [64] conv1_1 (fp32),
+ *                            shift / scale [3] the ScalingLayer; w_hi / w_lo / bias: HOST arrays of the other 12 convs in
+ *                            adb_conv3x3_bf16's weight layout; lin: HOST array of the 5 lin weights [C_l]; taps: NULL or a
+ *                            HOST array of 5 device buffers that receive each tap's fp32 NHWC features [2 n_frames,H_l,W_l,C_l]
+ *                            (NULL entries allowed).  lws: adb_lpips_workspace_bytes(n_frames, h, w)
+ *   adb_eval_reduce          table [T, ADB_EVAL_N_METRICS] (double) per view: PSNR, SSIM, LPIPS (NaN when with_lpips == 0),
+ *                            Render, GS, MSE, the five tap means.  PSNR / SSIM / LPIPS are the fp32 values the reference's
+ *                            .item() reads; every partial is added in a fixed order in double: bitwise reproducible */
+#define ADB_EVAL_N_METRICS 11
+int adb_eval_workspace_bytes(int T, int height, int width, long long n_gaussians, size_t* bytes /*HOST*/);
+int adb_eval_harmonize(int K, float* exposure, const uint8_t* is_test, int* n_bad, adb_stream_t stream);
+int adb_eval_count_visible(int T, int height, int width, long long n_gaussians, int t, const uint8_t* mask, void* ws,
+                           size_t ws_bytes, adb_stream_t stream);
+int adb_eval_image_metrics(int T, int height, int width, long long n_gaussians, const float* colors, const float* alphas,
+                           const float* exposure, const int* view_frame, const float* gt, float* image, float* ssim_map,
+                           void* ws, size_t ws_bytes, adb_stream_t stream);
+int adb_lpips_workspace_bytes(int n_frames, int height, int width, size_t* bytes /*HOST*/);
+int adb_lpips_vgg_forward(int T, int height, int width, long long n_gaussians, int frame0, int n_frames, const float* img0,
+                          const float* img1, const float* w1, const float* b1, const float* shift, const float* scale,
+                          const void* const* w_hi /*HOST*/, const void* const* w_lo /*HOST*/,
+                          const float* const* bias /*HOST*/, const float* const* lin /*HOST*/,
+                          float* const* taps /*HOST or NULL*/, void* lws, size_t lws_bytes, void* ews, size_t ews_bytes,
+                          adb_stream_t stream);
+int adb_eval_reduce(int T, int height, int width, long long n_gaussians, int with_lpips, void* ws, size_t ws_bytes,
+                    double* table, adb_stream_t stream);
+
 /* ---- map re-anchoring after the Backend moves its key frames (csrc/reanchor.cu) ----
  *   adb_reanchor_keyframes  replaces the pose loop of run_system.py:194-226 (pypose SE3 / quat2unit / mul / Inv / matrix,
  *                           Keyframe.get_Rt / set_Rt, three torch.linalg.inv per mapper key frame) for all K frames in one
