@@ -72,17 +72,16 @@ def lib() -> C.CDLL:
     return _lib
 
 
-# Kernel launches issued by one call of each entry point (CUB launches counted for scan/sort).
+# Kernel launches issued by one call of each entry point.
 LAUNCHES = {
-    "adb_ssim_forward": 1, "adb_ssim_backward": 1, "adb_raster_project_fwd": 1, "adb_raster_isect_scan": 2,
-    "adb_raster_isect_emit": 1, "adb_raster_sort": 8, "adb_raster_tile_offsets": 1, "adb_raster_blend_fwd": 1,
+    "adb_ssim_forward": 1, "adb_ssim_backward": 1, "adb_raster_project_fwd": 1, "adb_raster_blend_fwd": 1,
     "adb_raster_blend_bwd": 1, "adb_raster_project_bwd": 1,
-    "adb_raster_project_fwd_legacy": 1, "adb_raster_isect_emit_legacy": 1, "adb_raster_blend_fwd_legacy": 1,
-    "adb_raster_blend_bwd_legacy": 1, "adb_raster_tile_count_scan": 2, "adb_raster_tile_scatter_sort": 2,
+    "adb_raster_project_fwd_legacy": 1, "adb_raster_blend_fwd_legacy": 1,
+    "adb_raster_blend_bwd_legacy": 1, "adb_raster_tile_count_scan": 2,
     "adb_raster_blend_fwd_hits": 1, "adb_raster_blend_bwd_hits": 1,
     "adb_raster_project_bwd_multi": 1, "adb_raster_sh_bwd_multi": 1, "adb_raster_sh_dir_bwd_multi": 1,
     "adb_raster_sh_expand_multi": 1, "adb_raster_project_fwd_counts": 1, "adb_raster_tile_scan": 1,
-    "adb_raster_project_fwd_multi": 1, "adb_raster_tile_scan_multi": 1, "adb_raster_tile_scatter_sort_multi": 2,
+    "adb_raster_project_fwd_multi": 1, "adb_raster_tile_scan_multi": 1,
     "adb_raster_blend_fwd_multi": 1, "adb_raster_blend_bwd_multi": 1,
     "adb_raster_tile_band_scatter_sort": 3, "adb_raster_tile_band_scatter_sort_multi": 3,
 }

@@ -1,204 +1,49 @@
-// Tile intersection: scan of per-Gaussian tile counts, (key,value) emission, radix sort, tile ranges.
+// Tile intersection: for every tile, the depth-sorted list of the splats that touch it.
 // Integer / byte work with a BIT-EXACT contract against the oracle (SURVEY.md §8a R2c-R2e, App. B.3):
 //   key = (cam << (32+tile_bits)) | (tile << 32) | float_bits(depth),  val = cam*N + gaussian,
-//   emission order: Gaussian-major, then ty outer / tx inner; stable ascending sort over the live bits only.
+//   in the order of a stable ascending sort, over the live bits, of the keys emitted Gaussian-major, then ty outer / tx
+//   inner; tile_offsets[t] = the first sorted index of tile t, tile_offsets[T] = the number of intersections.
 // Replaces gsplat's isect_tiles / radix sort / isect_offset_encode that the reference reaches through
-// Reconstruct/scene/scene_models/h3dgsv3.py:664-680.
-//
-// Compiled with -fmad=false like raster_project.cu would not matter here (only /16, floor, ceil) but the tile
-// bound arithmetic below must stay textually identical to project_fwd_kernel's count.
-#include "raster_common.cuh"
-#include <cub/device/device_radix_sort.cuh>
-#include <cub/device/device_scan.cuh>
-#include <cub/iterator/transform_input_iterator.cuh>
-#include <stdio.h>
-
-namespace {
-
-struct ToI64 {
-    __host__ __device__ __forceinline__ int64_t operator()(const int32_t& v) const { return (int64_t)v; }
-};
-
-__global__ void __launch_bounds__(256)
-isect_emit_kernel(int N, const int32_t* __restrict__ radii, const float* __restrict__ splats,
-                  const int64_t* __restrict__ cum_tiles, int W, int H, int cam_id, int tile_bits, int convention,
-                  int64_t* __restrict__ keys, int32_t* __restrict__ vals) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= N) return;
-    const int2 r = reinterpret_cast<const int2*>(radii)[i];
-    if (r.x <= 0 && r.y <= 0) return;
-    const float4 rec0 = reinterpret_cast<const float4*>(splats + (size_t)i * ADB_SPLAT_STRIDE)[0];
-    const float depth = splats[(size_t)i * ADB_SPLAT_STRIDE + 11];
-    const int tw = (W + ADB_TILE - 1) / ADB_TILE;
-    int x0, x1, y0, y1;
-    adb_tile_rect(rec0.x, rec0.y, r.x, r.y, W, H, convention, x0, x1, y0, y1);
-    int64_t o = (i == 0) ? 0 : cum_tiles[i - 1];
-    if (convention != ADB_CONV_GSPLAT && cum_tiles[i] == o) return;  // kept its radius but was given no tiles
-    const uint64_t hi = (uint64_t)cam_id << (32 + tile_bits);
-    const uint64_t dbits = (uint64_t)__float_as_uint(depth);
-    const int32_t val = cam_id * N + i;
-    for (int ty = y0; ty < y1; ++ty)
-        for (int tx = x0; tx < x1; ++tx) {
-            uint64_t tile = (uint64_t)(ty * tw + tx);
-            keys[o] = (int64_t)(hi | (tile << 32) | dbits);
-            vals[o] = val;
-            ++o;
-        }
-}
-
-// offsets[t] = first sorted index whose tile id >= t; offsets[T] = n.
-__global__ void __launch_bounds__(256)
-tile_offsets_kernel(int64_t n, const int64_t* __restrict__ keys, int tile_bits, int T, int32_t* __restrict__ offsets) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const uint64_t mask = ((uint64_t)1 << tile_bits) - 1;
-    if (n == 0) {
-        if (i <= T) offsets[i] = 0;
-        return;
-    }
-    if (i >= n) return;
-    const int cur = (int)((((uint64_t)keys[i]) >> 32) & mask);
-    if (i == 0) {
-        for (int t = 0; t <= cur; ++t) offsets[t] = 0;
-    } else {
-        const int prev = (int)((((uint64_t)keys[i - 1]) >> 32) & mask);
-        for (int t = prev + 1; t <= cur; ++t) offsets[t] = (int32_t)i;
-    }
-    if (i == n - 1)
-        for (int t = cur + 1; t <= T; ++t) offsets[t] = (int32_t)n;
-}
-
-}  // namespace
-
-ADB_API int adb_raster_scan_workspace_bytes(int N, size_t* bytes) {
-    ADB_REQUIRE(bytes && N >= 0, "adb_raster_scan_workspace_bytes: bad args");
-    size_t b = 0;
-    cub::TransformInputIterator<int64_t, ToI64, const int32_t*> it((const int32_t*)nullptr, ToI64());
-    ADB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, b, it, (int64_t*)nullptr, N));
-    *bytes = b + 256;
-    return ADB_OK;
-}
-
-// cum_tiles[i] = sum_{j<=i} tiles_per_gauss[j]  (int64).  The caller reads cum_tiles[N-1] to size keys/vals.
-ADB_API int adb_raster_isect_scan(int N, const int32_t* tiles_per_gauss, int64_t* cum_tiles, void* ws,
-                                  size_t ws_bytes, cudaStream_t stream) {
-    ADB_REQUIRE(N >= 0, "adb_raster_isect_scan: bad N");
-    if (N == 0) return ADB_OK;
-    ADB_REQUIRE(tiles_per_gauss && cum_tiles && ws, "adb_raster_isect_scan: null pointer");
-    cub::TransformInputIterator<int64_t, ToI64, const int32_t*> it(tiles_per_gauss, ToI64());
-    size_t need = 0;
-    ADB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, need, it, cum_tiles, N));
-    if (need > ws_bytes) { adb_set_error_msg("adb_raster_isect_scan: workspace too small"); return ADB_ERR_WORKSPACE; }
-    ADB_CUDA(cub::DeviceScan::InclusiveSum(ws, need, it, cum_tiles, N, stream));
-    return ADB_OK;
-}
-
-static int isect_emit_impl(int convention, int N, const int32_t* radii, const float* splats, const int64_t* cum_tiles,
-                           int W, int H, int cam_id, int n_cams, int64_t* keys, int32_t* vals, cudaStream_t stream) {
-    ADB_REQUIRE(N >= 0 && W > 0 && H > 0 && cam_id >= 0 && n_cams > cam_id, "adb_raster_isect_emit: bad sizes");
-    if (N == 0) return ADB_OK;
-    ADB_REQUIRE(radii && splats && cum_tiles && keys && vals, "adb_raster_isect_emit: null pointer");
-    isect_emit_kernel<<<adb_cdiv(N, 256), 256, 0, stream>>>(N, radii, splats, cum_tiles, W, H, cam_id,
-                                                           adb_tile_bits(W, H), convention, keys, vals);
-    ADB_CHECK_LAUNCH("isect_emit_kernel");
-    return ADB_OK;
-}
-
-ADB_API int adb_raster_isect_emit(int N, const int32_t* radii, const float* splats, const int64_t* cum_tiles,
-                                  int W, int H, int cam_id, int n_cams, int64_t* keys, int32_t* vals,
-                                  cudaStream_t stream) {
-    return isect_emit_impl(ADB_CONV_GSPLAT, N, radii, splats, cum_tiles, W, H, cam_id, n_cams, keys, vals, stream);
-}
-
-// Legacy (Inria) tile rectangle; everything else (key layout, emission order) as above.
-ADB_API int adb_raster_isect_emit_legacy(int N, const int32_t* radii, const float* splats, const int64_t* cum_tiles,
-                                         int W, int H, int cam_id, int n_cams, int64_t* keys, int32_t* vals,
-                                         cudaStream_t stream) {
-    return isect_emit_impl(ADB_CONV_INRIA, N, radii, splats, cum_tiles, W, H, cam_id, n_cams, keys, vals, stream);
-}
-
-ADB_API int adb_raster_sort_workspace_bytes(long long n_isect, size_t* bytes) {
-    ADB_REQUIRE(bytes && n_isect >= 0, "adb_raster_sort_workspace_bytes: bad args");
-    size_t b = 0;
-    cub::DoubleBuffer<int64_t> dk(nullptr, nullptr);
-    cub::DoubleBuffer<int32_t> dv(nullptr, nullptr);
-    ADB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, b, dk, dv, (int64_t)n_isect, 0, 64));
-    *bytes = b + 256;
-    return ADB_OK;
-}
-
-// Stable ascending sort over the live key bits.  keys_a/vals_a hold the input; the sorted result lands in
-// whichever buffer pair *sorted_in_b reports (0 -> a, 1 -> b); both pairs must hold n_isect elements.
-ADB_API int adb_raster_sort(long long n_isect, int W, int H, int n_cams, int64_t* keys_a, int32_t* vals_a,
-                            int64_t* keys_b, int32_t* vals_b, void* ws, size_t ws_bytes, int* sorted_in_b,
-                            cudaStream_t stream) {
-    ADB_REQUIRE(n_isect >= 0 && sorted_in_b, "adb_raster_sort: bad args");
-    *sorted_in_b = 0;
-    if (n_isect == 0) return ADB_OK;
-    ADB_REQUIRE(keys_a && vals_a && keys_b && vals_b && ws, "adb_raster_sort: null pointer");
-    const int end_bit = 32 + adb_tile_bits(W, H) + adb_cam_bits(n_cams);
-    cub::DoubleBuffer<int64_t> dk(keys_a, keys_b);
-    cub::DoubleBuffer<int32_t> dv(vals_a, vals_b);
-    size_t need = 0;
-    ADB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, need, dk, dv, (int64_t)n_isect, 0, end_bit));
-    if (need > ws_bytes) { adb_set_error_msg("adb_raster_sort: workspace too small"); return ADB_ERR_WORKSPACE; }
-    ADB_CUDA(cub::DeviceRadixSort::SortPairs(ws, need, dk, dv, (int64_t)n_isect, 0, end_bit, stream));
-    *sorted_in_b = (dk.Current() == keys_b) ? 1 : 0;
-    return ADB_OK;
-}
-
-// tile_offsets has T+1 entries (T = ceil(W/16)*ceil(H/16)); entry T is n_isect.
-ADB_API int adb_raster_tile_offsets(long long n_isect, const int64_t* keys_sorted, int W, int H,
-                                    int32_t* tile_offsets, cudaStream_t stream) {
-    ADB_REQUIRE(n_isect >= 0 && W > 0 && H > 0 && tile_offsets, "adb_raster_tile_offsets: bad args");
-    ADB_REQUIRE(n_isect < 2147483647LL, "adb_raster_tile_offsets: more than 2^31 intersections");
-    const int T = adb_cdiv(W, ADB_TILE) * adb_cdiv(H, ADB_TILE);
-    long long threads = n_isect > 0 ? n_isect : (long long)T + 1;
-    tile_offsets_kernel<<<adb_cdiv(threads, 256), 256, 0, stream>>>(n_isect, keys_sorted, adb_tile_bits(W, H), T,
-                                                                   tile_offsets);
-    ADB_CHECK_LAUNCH("tile_offsets_kernel");
-    return ADB_OK;
-}
-
-
-// =====================================================================================================================
-// Tile-bucketed intersection (round 2): no library sort, no host sync, bit-identical output.
+// Reconstruct/scene/scene_models/h3dgsv3.py:664-680.  No library sort and no host sync:
 //
 //   count    per Gaussian: one RED.ADD per touched tile into tile_counts[tile][copy]            (16 B read / Gaussian)
-//   scan     one CTA: exclusive scan of the T x COPIES counters -> per-(tile,copy) segment starts + tile_offsets[T+1]
+//            (fused into the projection by adb_raster_project_fwd_counts / _multi; tile_count_kernel otherwise)
+//   scan     one CTA per view: exclusive scan of the T x COPIES counters -> per-(tile,copy) segment starts + tile_offsets[T+1]
 //            (clamped to the caller's capacity; the true total and an overflow flag stay on the device)
-//   scatter  per Gaussian: slot = start[tile][copy] + atomicSub(counter) - 1 -> packed[slot] = depth_bits<<32 | gaussian
-//            (arbitrary order inside a tile; the counters return to zero, so the buffer needs no memset between calls;
-//            four atomics are in flight per thread before the first dependent store)
+//   band     per chunk of 2048 Gaussians: one pair (word = depth_bits<<32 | gaussian, x0 | x1 << 16) per tile row the
+//            rectangle touches, counted per row in shared memory, one global atomic per (CTA, row) on the row's cursor, pairs
+//            grouped by row in shared memory and written as one run per row into the row's region of the scratch (the
+//            row's tile segments);
+//   expand   one CTA per (row, view): tile cursors in shared memory; per chunk of 1024 pairs the expanded words are
+//            grouped by tile in shared memory and written as one run per tile into `packed`; the row's counters are zeroed,
+//            so the buffer needs no memset between calls;
 //   sort     one CTA per tile: bitonic sort of the tile's 64-bit words — the 64-element sub-networks run in REGISTERS with
 //            warp shuffles, only the wider exchanges go through shared memory (global memory for tiles beyond 4096
 //            entries) — then keys = cam|tile|depth_bits and vals = cam*N + gaussian are written out.
 //
 // COPIES = 4 replicas of every tile counter (selected by CTA index) cut the same-address serialisation of the L2 atomics
-// that a single counter per tile suffers.
+// that a single counter per tile suffers.  The per-(tile, copy) counters are read only by the scan; the band pass uses one
+// cursor per row.  The band and expand passes store runs of consecutive slots: a scatter that stores each word where it
+// lands costs one returning L2 atomic and one stray 8-byte store per intersection, and its time follows the number of
+// those L2 requests rather than the bytes.
 //
-// Band scatter (adb_raster_tile_band_scatter_sort*, what raster.intersect / intersect_multi run): the scatter above does
-// one returning L2 atomic and one stray 8-byte store per intersection, each to a random place, and its time follows the
-// number of those L2 requests rather than the bytes.  The band scatter replaces it by two passes whose stores leave
-// shared memory as runs of consecutive slots:
-//   band pass  per chunk of 2048 Gaussians: one pair (word, x0 | x1 << 16) per tile row the rectangle touches, counted per
-//              row in shared memory, one global atomic per (CTA, row) on the row's cursor, pairs grouped by row in shared
-//              memory and written as one run per row into the row's region of the scratch (the row's tile segments);
-//   tile pass  one CTA per (row, view): tile cursors in shared memory; per chunk of 1024 pairs the expanded words are
-//              grouped by tile in shared memory and written as one run per tile into `packed`;
-//   sort       tile_sort_kernel as above.
-// Each tile receives the same words as from the scatter, so the sorted output is the same bit for bit.  The per-(tile,
-// copy) counters are read only by the scan; the band scatter uses one cursor per row.
-//
-// Views: the scan, scatter and sort take C views at once (one scan CTA per view, a view grid dimension for the scatter,
-// (T, C) CTAs for the sort).  View c has its own counter block [2*COPIES*T] and tile_offsets row [T+1], and owns the segment
+// Views: the scan, band, expand and sort take C views at once (one scan CTA per view, a view grid dimension for the
+// others).  View c has its own counter block [2*COPIES*T] and tile_offsets row [T+1], and owns the segment
 // [base_c, base_c + cap_c) of the one packed/keys/vals buffer, base_c = sum of the previous views' capacities.  Offsets and
 // vals are absolute in that buffer, so the blend kernels index it directly; vals follow gsplat's cam*N + gaussian.
 //
 // Why the order equals the reference's stable radix sort of (tile, depth): the reference emits keys Gaussian-major, so
 // inside one (tile, depth) tie the stable sort leaves ascending Gaussian ids — exactly the ascending order of the
 // composite word (depth_bits, gaussian).  A Gaussian touches a tile at most once, so the words of a tile are distinct
-// and the result does not depend on the scatter order.  (SURVEY.md App. B.3; oracle: adbo_isect_sort.)
-// The global 45-bit onesweep radix sort this replaces moved 6 x 24 B per intersection and was 12.6 % of the round-1 step.
+// and the result does not depend on the order in which the band and expand passes deliver them.  (SURVEY.md App. B.3;
+// oracle: adbo_isect_sort.)  A global 45-bit onesweep radix sort of the keys moved 6 x 24 B per intersection and was
+// 12.6 % of the round-1 step.
+//
+// Compiled with -fmad=false like raster_project.cu: it would not matter here (only /16, floor, ceil), but the tile
+// rectangle must stay the projection's (adb_tile_rect, raster_common.cuh).
+#include "raster_common.cuh"
+#include <stdio.h>
+
 namespace {
 
 constexpr int COPIES = ADB_TILE_COUNTER_COPIES;
@@ -305,48 +150,6 @@ tile_scan_kernel(int T, int32_t* __restrict__ counts_all, Segments seg, int32_t*
         if (offsets) offsets[T] = (int32_t)(seg_base + (tot < capacity ? tot : capacity));
         if (total) total[view] = tot;
         if (overflow && offsets && tot > capacity) overflow[view] = 1;
-    }
-}
-
-__global__ void __launch_bounds__(256)
-tile_scatter_kernel(int N, const int32_t* __restrict__ radii, const float* __restrict__ splats,
-                    const int32_t* __restrict__ tiles_per_gauss, int W, int H, int convention,
-                    int32_t* __restrict__ counts_all, Segments seg, unsigned long long* __restrict__ packed) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= N) return;
-    const int view = blockIdx.y;
-    const size_t vi = (size_t)view * N + i;
-    if (tiles_per_gauss[vi] <= 0) return;
-    const int2 r = reinterpret_cast<const int2*>(radii)[vi];
-    const float2 m = reinterpret_cast<const float2*>(splats + vi * ADB_SPLAT_STRIDE)[0];
-    const float depth = splats[vi * ADB_SPLAT_STRIDE + 11];
-    const int tw = (W + ADB_TILE - 1) / ADB_TILE;
-    const int T = tw * ((H + ADB_TILE - 1) / ADB_TILE);
-    int32_t* tile_counts = counts_all + (size_t)view * 2 * COPIES * T;
-    const int32_t* starts = tile_counts + (size_t)T * COPIES;
-    const long long seg_end = seg.base[view] + seg.cap[view];
-    const int cp = blockIdx.x & (COPIES - 1);
-    int x0, x1, y0, y1;
-    adb_tile_rect(m.x, m.y, r.x, r.y, W, H, convention, x0, x1, y0, y1);
-    const unsigned long long word = ((unsigned long long)__float_as_uint(depth) << 32) | (unsigned)i;
-    int tx = x0, ty = y0;
-    while (ty < y1) {
-        int e[4], a[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {                       // up to four atomics in flight
-            e[u] = -1;
-            if (ty < y1) {
-                e[u] = (ty * tw + tx) * COPIES + cp;
-                a[u] = atomicSub(tile_counts + e[u], 1);
-                if (++tx == x1) { tx = x0; ++ty; }
-            }
-        }
-#pragma unroll
-        for (int u = 0; u < 4; ++u)
-            if (e[u] >= 0) {
-                const long long slot = (long long)starts[e[u]] + (a[u] - 1);
-                if (slot < seg_end) packed[slot] = word;
-            }
     }
 }
 
@@ -836,21 +639,8 @@ static int scan_launch(int C, int T, int32_t* tile_counts, const Segments& seg, 
     return ADB_OK;
 }
 
-static int scatter_sort_launch(int N, int C, const int32_t* radii, const float* splats, const int32_t* tiles_per_gauss,
-                               int W, int H, int convention, int cam0, const Segments& seg, int32_t* tile_counts,
-                               const int32_t* tile_offsets, void* packed, int64_t* keys, int32_t* vals, cudaStream_t stream) {
-    const int T = adb_cdiv(W, ADB_TILE) * adb_cdiv(H, ADB_TILE);
-    tile_scatter_kernel<<<dim3(adb_cdiv(N, 256), C), 256, 0, stream>>>(N, radii, splats, tiles_per_gauss, W, H, convention,
-                                                                      tile_counts, seg, (unsigned long long*)packed);
-    ADB_CHECK_LAUNCH("tile_scatter_kernel");
-    tile_sort_kernel<<<dim3(T, C), SORT_THREADS, 0, stream>>>(T, tile_offsets, (unsigned long long*)packed, cam0, N,
-                                                             adb_tile_bits(W, H), keys, vals);
-    ADB_CHECK_LAUNCH("tile_sort_kernel");
-    return ADB_OK;
-}
-
 // tile_counts: int32 [2 * ADB_TILE_COUNTER_COPIES * T]: first half = the per-(tile,copy) counters, which must be all-zero
-// on entry (they are zero again after adb_raster_tile_scatter_sort: allocate + zero once); second half = segment starts
+// on entry (the expand pass of adb_raster_tile_band_scatter_sort zeroes them again); second half = segment starts
 // written by the scan.  tile_offsets [T+1]; total (int64, device) and overflow (int32, device, only ever SET) may be null.
 // `capacity` = number of elements `packed`, `keys` and `vals` can hold; intersections beyond it are dropped (memory-safe)
 // and flagged.
@@ -901,43 +691,6 @@ ADB_API int adb_raster_tile_scan_multi(int C, int W, int H, const long long* cap
     return scan_launch(C, T, tile_counts, seg, tile_offsets, total, overflow, stream);
 }
 
-// Scatter + per-tile sort.  keys [capacity] int64, vals [capacity] int32, packed [capacity] uint64 scratch; tile_counts as
-// left by adb_raster_tile_count_scan.
-ADB_API int adb_raster_tile_scatter_sort(int N, const int32_t* radii, const float* splats, const int32_t* tiles_per_gauss,
-                                         int W, int H, int legacy, int cam_id, int n_cams, long long capacity,
-                                         int32_t* tile_counts, const int32_t* tile_offsets, void* packed, int64_t* keys,
-                                         int32_t* vals, cudaStream_t stream) {
-    ADB_REQUIRE(N >= 0 && W > 0 && H > 0 && cam_id >= 0 && n_cams > cam_id && capacity >= 0,
-                "adb_raster_tile_scatter_sort: bad sizes");
-    if (N == 0 || capacity == 0) return ADB_OK;
-    ADB_REQUIRE(radii && splats && tiles_per_gauss && tile_counts && tile_offsets && packed && keys && vals,
-                "adb_raster_tile_scatter_sort: null pointer");
-    ADB_REQUIRE(capacity < 2147483647LL, "adb_raster_tile_scatter_sort: bad sizes");
-    Segments seg;
-    seg.base[0] = 0;
-    seg.cap[0] = capacity;
-    return scatter_sort_launch(N, 1, radii, splats, tiles_per_gauss, W, H, legacy ? ADB_CONV_INRIA : ADB_CONV_GSPLAT, cam_id,
-                               seg, tile_counts, tile_offsets, packed, keys, vals, stream);
-}
-
-// C views in one scatter and one sort launch: radii [C,N,2], splats [C,N,12], tiles_per_gauss [C,N]; tile_counts and
-// tile_offsets as left by adb_raster_tile_scan_multi with the SAME host capacities [C].  packed / vals (and keys unless
-// NULL) hold sum(capacities) elements; view c's entries start at the sum of the previous capacities, vals = c*N + gaussian.
-ADB_API int adb_raster_tile_scatter_sort_multi(int N, int C, const int32_t* radii, const float* splats,
-                                               const int32_t* tiles_per_gauss, int W, int H, const long long* capacities,
-                                               int32_t* tile_counts, const int32_t* tile_offsets, void* packed,
-                                               int64_t* keys, int32_t* vals, cudaStream_t stream) {
-    Segments seg;
-    const int rc = make_segments("adb_raster_tile_scatter_sort_multi", C, capacities, seg);
-    if (rc != ADB_OK) return rc;
-    ADB_REQUIRE(N >= 0 && W > 0 && H > 0 && (long long)C * N < 2147483647LL, "adb_raster_tile_scatter_sort_multi: bad sizes");
-    if (N == 0) return ADB_OK;
-    ADB_REQUIRE(radii && splats && tiles_per_gauss && tile_counts && tile_offsets && packed && vals,
-                "adb_raster_tile_scatter_sort_multi: null pointer");
-    return scatter_sort_launch(N, C, radii, splats, tiles_per_gauss, W, H, ADB_CONV_GSPLAT, 0, seg, tile_counts, tile_offsets,
-                               packed, keys, vals, stream);
-}
-
 // Pair words (8 B) and pair columns (4 B) per slot of the intersection buffer.
 ADB_API int adb_raster_tile_band_scratch_bytes(long long capacity, size_t* bytes) {
     ADB_REQUIRE(bytes && capacity >= 0 && capacity < 2147483647LL, "adb_raster_tile_band_scratch_bytes: bad args");
@@ -982,7 +735,8 @@ static int band_scatter_sort_launch(const char* name, int N, int C, const int32_
     return ADB_OK;
 }
 
-// adb_raster_tile_scatter_sort with the band scatter; scratch from adb_raster_tile_band_scratch_bytes(capacity).
+// Band and expand passes + per-tile sort.  keys [capacity] int64, vals [capacity] int32, packed [capacity] uint64 and
+// scratch (adb_raster_tile_band_scratch_bytes(capacity)) scratch; tile_counts as left by adb_raster_tile_count_scan.
 ADB_API int adb_raster_tile_band_scatter_sort(int N, const int32_t* radii, const float* splats,
                                               const int32_t* tiles_per_gauss, int W, int H, int legacy, int cam_id,
                                               int n_cams, long long capacity, int32_t* tile_counts,
@@ -999,8 +753,10 @@ ADB_API int adb_raster_tile_band_scatter_sort(int N, const int32_t* radii, const
                                     packed, scratch, scratch_bytes, keys, vals, stream);
 }
 
-// adb_raster_tile_scatter_sort_multi with the band scatter; scratch from adb_raster_tile_band_scratch_bytes(sum of the
-// capacities).
+// C views in one launch per pass: radii [C,N,2], splats [C,N,12], tiles_per_gauss [C,N]; tile_counts and tile_offsets as
+// left by adb_raster_tile_scan_multi with the SAME host capacities [C].  packed / vals (and keys unless NULL) hold
+// sum(capacities) elements, scratch adb_raster_tile_band_scratch_bytes(sum(capacities)) bytes; view c's entries start at
+// the sum of the previous capacities, vals = c*N + gaussian.
 ADB_API int adb_raster_tile_band_scatter_sort_multi(int N, int C, const int32_t* radii, const float* splats,
                                                     const int32_t* tiles_per_gauss, int W, int H,
                                                     const long long* capacities, int32_t* tile_counts,

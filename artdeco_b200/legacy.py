@@ -11,7 +11,7 @@ sh_degree, campos[3], prefiltered, debug)`` and the call
 ``means2D`` is the usual gradient holder: after backward its ``.grad[:, :2]`` holds dL/d(mean2D) in the Inria NDC scaling
 (pixel gradient x 0.5*W, 0.5*H).
 
-All compute goes through the C ABI (adb_raster_*_legacy + the shared scan / sort / tile_offsets / project_bwd).
+All compute goes through the C ABI (adb_raster_*_legacy + the shared tile intersection and project_bwd).
 """
 from __future__ import annotations
 

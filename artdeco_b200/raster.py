@@ -23,14 +23,7 @@ _lib.register("adb_raster_project_fwd", [i32, vp, vp, vp, vp, vp, i32, vp, vp, v
 _lib.register("adb_raster_project_fwd_counts", [i32, vp, vp, vp, vp, vp, i32, vp, vp, vp, i32, i32, f32, f32, f32, f32,
                                                 vp, vp, vp, vp, vp])
 _lib.register("adb_raster_tile_scan", [i32, i32, i64, vp, vp, vp, vp, vp])
-_lib.register("adb_raster_scan_workspace_bytes", [i32, C.POINTER(C.c_size_t)])
-_lib.register("adb_raster_isect_scan", [i32, vp, vp, vp, C.c_size_t, vp])
-_lib.register("adb_raster_isect_emit", [i32, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp])
-_lib.register("adb_raster_sort_workspace_bytes", [i64, C.POINTER(C.c_size_t)])
-_lib.register("adb_raster_sort", [i64, i32, i32, i32, vp, vp, vp, vp, vp, C.c_size_t, C.POINTER(C.c_int), vp])
-_lib.register("adb_raster_tile_offsets", [i64, vp, i32, i32, vp, vp])
 _lib.register("adb_raster_tile_count_scan", [i32, vp, vp, vp, i32, i32, i32, i64, vp, vp, vp, vp, vp])
-_lib.register("adb_raster_tile_scatter_sort", [i32, vp, vp, vp, i32, i32, i32, i32, i32, i64, vp, vp, vp, vp, vp, vp])
 _lib.register("adb_raster_tile_band_scratch_bytes", [i64, C.POINTER(C.c_size_t)])
 _lib.register("adb_raster_tile_band_scatter_sort", [i32, vp, vp, vp, i32, i32, i32, i32, i32, i64, vp, vp, vp, vp,
                                                     C.c_size_t, vp, vp, vp])
@@ -46,7 +39,6 @@ _lib.register("adb_raster_sh_expand_multi", [i32, i32, vp, i32, vp, vp, vp, vp])
 
 _lib.register("adb_raster_project_fwd_legacy", [i32, vp, vp, vp, vp, vp, i32, vp, vp, vp, i32, i32, f32, f32, f32,
                                                 vp, vp, vp, vp])
-_lib.register("adb_raster_isect_emit_legacy", [i32, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp])
 _lib.register("adb_raster_blend_fwd_hits", [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp])
 _lib.register("adb_raster_blend_bwd_hits", [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp])
 _lib.register("adb_raster_blend_fwd_legacy", [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp])
@@ -56,7 +48,6 @@ _caps_t = C.POINTER(C.c_longlong)
 _lib.register("adb_raster_project_fwd_multi", [i32, i32, vp, vp, vp, vp, vp, i32, vp, vp, vp, i32, i32, f32, f32, f32, f32,
                                                vp, vp, vp, vp, vp])
 _lib.register("adb_raster_tile_scan_multi", [i32, i32, i32, _caps_t, vp, vp, vp, vp, vp])
-_lib.register("adb_raster_tile_scatter_sort_multi", [i32, i32, vp, vp, vp, i32, i32, _caps_t, vp, vp, vp, vp, vp, vp])
 _lib.register("adb_raster_tile_band_scatter_sort_multi", [i32, i32, vp, vp, vp, i32, i32, _caps_t, vp, vp, vp, vp,
                                                           C.c_size_t, vp, vp, vp])
 _lib.register("adb_raster_blend_fwd_multi", [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp])
@@ -66,17 +57,6 @@ _lib.register("adb_raster_blend_bwd_multi", [i32, i32, i32, i32, vp, vp, vp, vp,
 TILE = 16
 SPLAT_STRIDE = 12
 COUNTER_COPIES = 4      # ADB_TILE_COUNTER_COPIES (csrc/raster_common.cuh)
-
-_ws_cache: dict = {}
-
-
-def _workspace(dev: torch.device, nbytes: int) -> torch.Tensor:
-    key = (dev.index, "ws")
-    t = _ws_cache.get(key)
-    if t is None or t.numel() < nbytes:
-        t = torch.empty(max(nbytes, 1 << 20), dtype=torch.uint8, device=dev)
-        _ws_cache[key] = t
-    return t
 
 
 def _f32c(t: torch.Tensor) -> torch.Tensor:
@@ -249,12 +229,9 @@ def blend_backward_multi(W, H, splats, vals, offsets, alphas, last_ids, v_colors
     return v_splats
 
 
-def intersect(radii, splats, tpg, W, H, cam_id=0, n_cams=1, sort=True, legacy=False, capacity=None, method=None, counts=None):
-    """Tile keys/values (sorted), tile offsets [T+1] for one camera.
-
-    ``method="bucket"`` (default): tile-bucketed pipeline — count, scan, band scatter, one CTA-local bitonic sort per tile
-    (csrc/raster_isect.cu) — bit-identical to the stable radix sort of (cam | tile | depth) keys it replaces.
-    ``method="radix"`` (or env ADB_ISECT=radix): round-1 path (scan, emit, CUB onesweep radix sort, offsets), kept for A/B.
+def intersect(radii, splats, tpg, W, H, cam_id=0, n_cams=1, legacy=False, capacity=None, counts=None):
+    """Tile keys/values (sorted), tile offsets [T+1] for one camera: count, scan, band scatter, one CTA-local bitonic sort
+    per tile (csrc/raster_isect.cu), bit-identical to the stable radix sort of (cam | tile | depth) keys.
 
     ``capacity=None``: one host sync to size keys/vals exactly (gsplat does the same: ``cum_tiles[-1].item()``);
     returns ``(keys[I], vals[I], offsets, I:int)``.
@@ -266,9 +243,6 @@ def intersect(radii, splats, tpg, W, H, cam_id=0, n_cams=1, sort=True, legacy=Fa
     N = radii.shape[0]
     dev = radii.device
     T = ((W + TILE - 1) // TILE) * ((H + TILE - 1) // TILE)
-    if method is None:
-        import os
-        method = os.environ.get("ADB_ISECT", "bucket")
     offsets = torch.empty(T + 1, dtype=torch.int32, device=dev)
     if N == 0:
         offsets.zero_()
@@ -278,62 +252,36 @@ def intersect(radii, splats, tpg, W, H, cam_id=0, n_cams=1, sort=True, legacy=Fa
             return e64, e32, offsets, 0
         return e64, e32, offsets, {"n_isect": torch.zeros(1, dtype=torch.int64, device=dev),
                                    "overflow": torch.zeros(1, dtype=torch.int32, device=dev)}
-    if method == "bucket" and sort:
-        total = torch.zeros(1, dtype=torch.int64, device=dev)
-        overflow = torch.zeros(1, dtype=torch.int32, device=dev)
-        cap_scan = int(capacity) if capacity is not None else 2147483646
-        if counts is not None:
-            _lib.call("adb_raster_tile_scan", W, H, cap_scan, _lib.ptr(counts), _lib.ptr(offsets), _lib.ptr(total),
-                      _lib.ptr(overflow), _lib.stream())
-        else:
-            counts = torch.zeros(2 * COUNTER_COPIES * T, dtype=torch.int32, device=dev)   # counters | segment starts
-            _lib.call("adb_raster_tile_count_scan", N, _lib.ptr(radii), _lib.ptr(splats), _lib.ptr(tpg), W, H, int(legacy),
-                      cap_scan, _lib.ptr(counts), _lib.ptr(offsets), _lib.ptr(total), _lib.ptr(overflow), _lib.stream())
-        if capacity is None:
-            n_isect = int(total.item())      # the pipeline's single host sync
-            if n_isect >= 2147483647:
-                raise _lib.ArtdecoB200Error("more than 2^31 tile intersections")
-            cap = n_isect
-        else:
-            cap = int(capacity)
-        keys = torch.empty(max(cap, 1), dtype=torch.int64, device=dev)
-        vals = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
-        if cap > 0:
-            packed = torch.empty(cap, dtype=torch.int64, device=dev)
-            scratch = band_scratch(cap, dev)
-            _lib.call("adb_raster_tile_band_scatter_sort", N, _lib.ptr(radii), _lib.ptr(splats), _lib.ptr(tpg), W, H,
-                      int(legacy), cam_id, n_cams, cap, _lib.ptr(counts), _lib.ptr(offsets), _lib.ptr(packed),
-                      _lib.ptr(scratch), scratch.numel(), _lib.ptr(keys), _lib.ptr(vals), _lib.stream())
-        else:
-            counts.zero_()
-        if capacity is None:
-            return keys[:n_isect], vals[:n_isect], offsets, n_isect
-        return keys[:cap], vals[:cap], offsets, {"n_isect": total, "overflow": overflow}
-    if capacity is not None:
-        raise NotImplementedError("capacity mode needs method='bucket'")
-    nb = C.c_size_t(0)
-    _lib.call("adb_raster_scan_workspace_bytes", N, C.byref(nb))
-    cum = torch.empty(N, dtype=torch.int64, device=dev)
-    ws = _workspace(dev, nb.value)
-    _lib.call("adb_raster_isect_scan", N, _lib.ptr(tpg), _lib.ptr(cum), _lib.ptr(ws), ws.numel(), _lib.stream())
-    n_isect = int(cum[-1].item())  # the pipeline's single host sync
-    keys_a = torch.empty(max(n_isect, 1), dtype=torch.int64, device=dev)
-    vals_a = torch.empty(max(n_isect, 1), dtype=torch.int32, device=dev)
-    if n_isect > 0:
-        _lib.call("adb_raster_isect_emit_legacy" if legacy else "adb_raster_isect_emit", N, _lib.ptr(radii), _lib.ptr(splats), _lib.ptr(cum), W, H, cam_id, n_cams,
-                  _lib.ptr(keys_a), _lib.ptr(vals_a), _lib.stream())
-    keys, vals = keys_a, vals_a
-    if sort and n_isect > 0:
-        keys_b, vals_b = torch.empty_like(keys_a), torch.empty_like(vals_a)
-        _lib.call("adb_raster_sort_workspace_bytes", n_isect, C.byref(nb))
-        ws = _workspace(dev, nb.value)
-        in_b = C.c_int(0)
-        _lib.call("adb_raster_sort", n_isect, W, H, n_cams, _lib.ptr(keys_a), _lib.ptr(vals_a), _lib.ptr(keys_b),
-                  _lib.ptr(vals_b), _lib.ptr(ws), ws.numel(), C.byref(in_b), _lib.stream())
-        if in_b.value:
-            keys, vals = keys_b, vals_b
-    _lib.call("adb_raster_tile_offsets", n_isect, _lib.ptr(keys), W, H, _lib.ptr(offsets), _lib.stream())
-    return keys[:n_isect], vals[:n_isect], offsets, n_isect
+    total = torch.zeros(1, dtype=torch.int64, device=dev)
+    overflow = torch.zeros(1, dtype=torch.int32, device=dev)
+    cap_scan = int(capacity) if capacity is not None else 2147483646
+    if counts is not None:
+        _lib.call("adb_raster_tile_scan", W, H, cap_scan, _lib.ptr(counts), _lib.ptr(offsets), _lib.ptr(total),
+                  _lib.ptr(overflow), _lib.stream())
+    else:
+        counts = torch.zeros(2 * COUNTER_COPIES * T, dtype=torch.int32, device=dev)   # counters | segment starts
+        _lib.call("adb_raster_tile_count_scan", N, _lib.ptr(radii), _lib.ptr(splats), _lib.ptr(tpg), W, H, int(legacy),
+                  cap_scan, _lib.ptr(counts), _lib.ptr(offsets), _lib.ptr(total), _lib.ptr(overflow), _lib.stream())
+    if capacity is None:
+        n_isect = int(total.item())      # the pipeline's single host sync
+        if n_isect >= 2147483647:
+            raise _lib.ArtdecoB200Error("more than 2^31 tile intersections")
+        cap = n_isect
+    else:
+        cap = int(capacity)
+    keys = torch.empty(max(cap, 1), dtype=torch.int64, device=dev)
+    vals = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
+    if cap > 0:
+        packed = torch.empty(cap, dtype=torch.int64, device=dev)
+        scratch = band_scratch(cap, dev)
+        _lib.call("adb_raster_tile_band_scatter_sort", N, _lib.ptr(radii), _lib.ptr(splats), _lib.ptr(tpg), W, H,
+                  int(legacy), cam_id, n_cams, cap, _lib.ptr(counts), _lib.ptr(offsets), _lib.ptr(packed),
+                  _lib.ptr(scratch), scratch.numel(), _lib.ptr(keys), _lib.ptr(vals), _lib.stream())
+    else:
+        counts.zero_()
+    if capacity is None:
+        return keys[:n_isect], vals[:n_isect], offsets, n_isect
+    return keys[:cap], vals[:cap], offsets, {"n_isect": total, "overflow": overflow}
 
 
 def new_hit_mask(vals: torch.Tensor):

@@ -192,16 +192,6 @@ int adb_raster_project_fwd_multi(int N, int C, const float* means, const float* 
                                  const float* Ks, const float* camposs, int W, int H, float eps2d, float near_plane,
                                  float far_plane, float radius_clip, int32_t* radii, float* splats,
                                  int32_t* tiles_per_gauss, int32_t* tile_counts, adb_stream_t stream);
-int adb_raster_scan_workspace_bytes(int N, size_t* bytes /*HOST*/);
-int adb_raster_isect_scan(int N, const int32_t* tiles_per_gauss, int64_t* cum_tiles /*[N] inclusive*/, void* ws,
-                          size_t ws_bytes, adb_stream_t stream);
-int adb_raster_isect_emit(int N, const int32_t* radii, const float* splats, const int64_t* cum_tiles, int W, int H,
-                          int cam_id, int n_cams, int64_t* keys, int32_t* vals, adb_stream_t stream);
-int adb_raster_sort_workspace_bytes(long long n_isect, size_t* bytes /*HOST*/);
-int adb_raster_sort(long long n_isect, int W, int H, int n_cams, int64_t* keys_a, int32_t* vals_a, int64_t* keys_b,
-                    int32_t* vals_b, void* ws, size_t ws_bytes, int* sorted_in_b /*HOST*/, adb_stream_t stream);
-int adb_raster_tile_offsets(long long n_isect, const int64_t* keys_sorted, int W, int H,
-                            int32_t* tile_offsets /*[T+1]*/, adb_stream_t stream);
 /* Multi-view backward (BASELINE config 4: C views of the same Gaussians per optimiser step; csrc/raster_project_bwd_multi.cu).
  * Same mathematics as C calls of adb_raster_project_bwd summed (gsplat's fully_fused_projection_bwd + spherical_harmonics_bwd
  * under autograd's accumulation, h3dgsv3.py:664-680), with parameters read once and every gradient written once.
@@ -227,45 +217,39 @@ int adb_raster_sh_dir_bwd_multi(int N, int C, const float* means, const float* s
                                 const float* splats, const float* v_splats, float* v_means, float* v_campos, adb_stream_t stream);
 int adb_raster_sh_expand_multi(int N, int C, const float* means, int sh_degree, const float* campos, const float* g_rgb,
                                float* v_sh, adb_stream_t stream);
-/* Tile-bucketed intersection (no library sort, no host sync; bit-identical to adb_raster_isect_emit + adb_raster_sort +
- * adb_raster_tile_offsets, i.e. to gsplat's isect_tiles / radix sort / isect_offset_encode behind h3dgsv3.py:664-680):
+/* Tile intersection (no library sort, no host sync; csrc/raster_isect.cu): bit-identical to gsplat's isect_tiles / radix
+ * sort / isect_offset_encode behind h3dgsv3.py:664-680 — keys = cam|tile|depth_bits, vals = cam*N + gaussian, in the order
+ * of a stable sort of the keys emitted Gaussian-major (oracle/raster_oracle.c, adbo_isect_sort).
  *   adb_raster_tile_count_scan   per-tile counts (RED.ADD) + one-CTA exclusive scan -> tile_offsets[T+1] clamped to
  *                                `capacity`; *total (int64, device) = true intersection count, *overflow (int32, device)
  *                                is SET when total > capacity.  tile_counts: int32[2*4*T] (4 replicated counters per tile,
  *                                then their segment starts); the first half must be zero on entry.
- *   adb_raster_tile_scatter_sort scatter depth_bits<<32|gaussian into each tile's segment (counters return to zero), then
- *                                one CTA per tile sorts its segment (bitonic, shared memory; global memory beyond 4096
- *                                entries) and writes keys = cam|tile|depth_bits, vals = cam*N + gaussian.
- * packed: uint64[capacity] scratch.  legacy != 0 selects the Inria tile rectangle. */
+ *   adb_raster_tile_scan         the scan alone, for counters filled by adb_raster_project_fwd_counts.
+ *   adb_raster_tile_band_scatter_sort
+ *     band pass  one (Gaussian, tile row) pair per tile row a splat touches, appended per CTA in runs to the row's region
+ *                of `scratch` (the row's tile segments; pairs of a row cut by the capacity are rebuilt from the splats);
+ *     tile pass  one CTA per (tile row, view) expands the row's pairs into its tiles' segments of `packed` and zeroes the
+ *                row's counters;
+ *     sort       one CTA per tile sorts its segment (bitonic, shared memory; global memory beyond 4096 entries) and writes
+ *                keys and vals.
+ *     packed: uint64[capacity]; scratch: adb_raster_tile_band_scratch_bytes(capacity) bytes; neither needs initialisation.
+ *     tile_counts as left by the scan: its per-tile segment starts are used, and overwritten, as per-row cursors, and its
+ *     first half is zero again after a call that launches (N > 0 and capacity > 0).  W and H at most 65536 (4096 tiles).
+ * legacy != 0 selects the Inria tile rectangle. */
 int adb_raster_tile_count_scan(int N, const int32_t* radii, const float* splats, const int32_t* tiles_per_gauss, int W, int H,
                                int legacy, long long capacity, int32_t* tile_counts, int32_t* tile_offsets, long long* total,
                                int32_t* overflow, adb_stream_t stream);
 int adb_raster_tile_scan(int W, int H, long long capacity, int32_t* tile_counts, int32_t* tile_offsets, long long* total,
                          int32_t* overflow, adb_stream_t stream);
-int adb_raster_tile_scatter_sort(int N, const int32_t* radii, const float* splats, const int32_t* tiles_per_gauss, int W, int H,
-                                 int legacy, int cam_id, int n_cams, long long capacity, int32_t* tile_counts,
-                                 const int32_t* tile_offsets, void* packed, int64_t* keys, int32_t* vals, adb_stream_t stream);
 /* View-batched intersection (one launch per stage for C views; 1 <= C <= 64).  capacities: HOST array [C]; view c owns the
  * segment [sum_{c'<c} capacities[c'], +capacities[c]) of one packed / keys / vals buffer (the sum must stay below 2^31 - 1).
- *   adb_raster_tile_scan_multi         one CTA per view: tile_offsets [C,T+1] ABSOLUTE in that buffer, clamped to the view's
- *                                      capacity; total int64 [C] and overflow int32 [C] (SET when total[c] > capacities[c])
- *                                      on the device.  tile_offsets == NULL: totals only (a sizing pass).
- *   adb_raster_tile_scatter_sort_multi scatter (view grid dimension) + per-tile sort over (T, C) CTAs; vals = c*N + gaussian;
- *                                      keys (may be NULL: not written) = c|tile|depth_bits as adb_raster_tile_scatter_sort. */
+ *   adb_raster_tile_scan_multi              one CTA per view: tile_offsets [C,T+1] ABSOLUTE in that buffer, clamped to the
+ *                                           view's capacity; total int64 [C] and overflow int32 [C] (SET when total[c] >
+ *                                           capacities[c]) on the device.  tile_offsets == NULL: totals only (a sizing pass).
+ *   adb_raster_tile_band_scatter_sort_multi the three passes above with a view grid dimension; scratch for the sum of the
+ *                                           capacities; vals = c*N + gaussian; keys (may be NULL: not written) = c|tile|depth_bits. */
 int adb_raster_tile_scan_multi(int C, int W, int H, const long long* capacities /*HOST [C]*/, int32_t* tile_counts,
                                int32_t* tile_offsets, long long* total, int32_t* overflow, adb_stream_t stream);
-int adb_raster_tile_scatter_sort_multi(int N, int C, const int32_t* radii, const float* splats, const int32_t* tiles_per_gauss,
-                                       int W, int H, const long long* capacities /*HOST [C]*/, int32_t* tile_counts,
-                                       const int32_t* tile_offsets, void* packed, int64_t* keys, int32_t* vals,
-                                       adb_stream_t stream);
-/* Band scatter: the same results as adb_raster_tile_scatter_sort(_multi), bit for bit, with the scatter's writes in runs.
- *   band pass  one (Gaussian, tile row) pair per tile row a splat touches, appended per CTA in runs to the row's region
- *              of `scratch` (the row's tile segments; pairs of a row cut by the capacity are rebuilt from the splats);
- *   tile pass  one CTA per (tile row, view) expands the row's pairs into its tiles' segments of `packed`;
- *   sort       as adb_raster_tile_scatter_sort.
- * scratch: adb_raster_tile_band_scratch_bytes(sum of the capacities) bytes, no initialisation.  tile_counts as left by the
- * scan (the first half returns to zero); its per-tile segment starts are used, and overwritten, as per-row cursors.
- * W and H at most 65536 (4096 tiles). */
 int adb_raster_tile_band_scratch_bytes(long long capacity, size_t* bytes);
 int adb_raster_tile_band_scatter_sort(int N, const int32_t* radii, const float* splats, const int32_t* tiles_per_gauss, int W,
                                       int H, int legacy, int cam_id, int n_cams, long long capacity, int32_t* tile_counts,
@@ -315,14 +299,13 @@ int adb_raster_project_bwd(int N, const float* means, const float* quats, const 
  * Reconstruct/webviewer/scene_models.py:559-605 (SURVEY.md §8a R3; the fork itself is not vendored, so the constants are
  * the published Inria ones: radius ceil(3 sqrt(lambda_max)), +0.3 px^2 low-pass (pass eps2d = 0.3), near 0.2, alpha <= 0.99,
  * stop at T(1-alpha) < 1e-4, tile rectangle (int)((p-r)/16)..(int)((p+r+15)/16) on pixel-index coordinates).
- * Same buffers and key layout as the gsplat-convention entry points above; scan / sort / tile_offsets / project_bwd are shared. */
+ * Same buffers and key layout as the gsplat-convention entry points above; the tile intersection (legacy = 1) and
+ * project_bwd are shared. */
 int adb_raster_project_fwd_legacy(int N, const float* means, const float* quats, const float* scales,
                                   const float* opacities, const float* sh, int sh_degree, const float* viewmat,
                                   const float* K, const float* campos, int W, int H, float eps2d, float near_plane,
                                   float far_plane, int32_t* radii /*[N,2], both = Inria radius*/, float* splats,
                                   int32_t* tiles_per_gauss, adb_stream_t stream);
-int adb_raster_isect_emit_legacy(int N, const int32_t* radii, const float* splats, const int64_t* cum_tiles, int W, int H,
-                                 int cam_id, int n_cams, int64_t* keys, int32_t* vals, adb_stream_t stream);
 int adb_raster_blend_fwd_legacy(int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
                                 const int32_t* tile_offsets, float* colors /*[H,W,4]: rgb, sum alpha*T/z*/, float* alphas,
                                 int32_t* last_ids, int32_t* main_ids /*[H,W] argmax alpha*T, -1 none; may be NULL*/,

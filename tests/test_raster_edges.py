@@ -416,9 +416,6 @@ def test_intersection_ladder_bit_exact(cuda, regime):
 
     assert g["n"] == n
     same(g["keys"], g["vals"], g["offs"], "bucketed")
-    kr, vr, orr, nr = R.intersect(g["radii"], g["splats"], g["tpg"], W, H, method="radix")
-    assert nr == n
-    same(kr, vr, orr, "radix")
     for cap in (n, n + 4321):
         k2, v2, o2, info = R.intersect(g["radii"], g["splats"], g["tpg"], W, H, capacity=cap)
         assert int(info["n_isect"]) == n and int(info["overflow"]) == 0, cap
@@ -631,7 +628,7 @@ VARIANTS = {"tma": {"ADB_BLEND_TMA": "1"}, "slots32": {"ADB_BWD_SLOTS": "32"}, "
 # 32 slots also reassociate each warp's 32-pixel moment sums (one pass instead of two 16-pixel halves and a shuffle), and
 # the conversion to splat-centred moments (ex (ex S0 - 2 Sx) + Sxx, ex up to 8 px) amplifies that rounding
 BWD_BOUND = {"tma": 2e-6, "slots32": 2e-5, "occ3": 2e-6}
-SWITCHES = ("ADB_BLEND_TMA", "ADB_BWD_SLOTS", "ADB_BWD_OCC", "ADB_BLEND_HITS", "ADB_ISECT")
+SWITCHES = ("ADB_BLEND_TMA", "ADB_BWD_SLOTS", "ADB_BWD_OCC", "ADB_BLEND_HITS")
 
 
 @functools.lru_cache(maxsize=None)

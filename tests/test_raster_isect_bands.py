@@ -1,8 +1,9 @@
 """The band scatter of the tile intersection (adb_raster_tile_band_scatter_sort and its multi-view form): sorted values,
 keys, offsets, totals and overflow flags against the C oracle at the edges of its two passes — empty tile rows, views with
 nothing visible, N = 0 and 1, a splat covering every tile row, a tile beyond the shared-memory sort, frames that are not a
-multiple of the tile, the Inria rectangle, C = 1 and 8, and capacities cut on and inside a tile row, with canary words
-past every buffer.  Also: two runs are bitwise equal, and a graph replay equals the eager call."""
+multiple of the tile, the Inria rectangle (against the PyTorch reference), C = 1 and 8, and capacities cut on and inside
+a tile row, with canary words past every buffer.  Also: two runs are bitwise equal, and a graph replay equals the eager
+call."""
 import ctypes
 
 import numpy as np
@@ -11,6 +12,7 @@ import torch
 
 import oracle
 from artdeco_b200 import synthetic
+from oracle import legacy_torch, raster_torch
 
 TILE = 16
 CANARY = 0x5A5A5A5A
@@ -98,6 +100,7 @@ def test_band_entry_points_refuse_bad_arguments_before_touching_the_device():
 
     dummy = ctypes.c_void_p(16)
     caps = (ctypes.c_longlong * 2)(100, 100)
+    huge = (ctypes.c_longlong * 2)(2_000_000_000, 2_000_000_000)     # the int32 offsets cannot address their sum
     nb = ctypes.c_size_t(0)
     assert L.adb_raster_tile_band_scratch_bytes(100, ctypes.byref(nb)) == 0 and nb.value == 1200
     assert refused(L.adb_raster_tile_band_scratch_bytes(-1, ctypes.byref(nb)), "adb_raster_tile_band_scratch_bytes")
@@ -113,8 +116,12 @@ def test_band_entry_points_refuse_bad_arguments_before_touching_the_device():
     sm = L.adb_raster_tile_band_scatter_sort_multi
     assert refused(sm(8, 0, dummy, dummy, dummy, 64, 64, caps, dummy, dummy, dummy, dummy, 2400, None, dummy, None),
                    "adb_raster_tile_band_scatter_sort_multi")
+    assert refused(sm(8, 2, dummy, dummy, dummy, 64, 64, huge, dummy, dummy, dummy, dummy, 2400, None, dummy, None),
+                   "adb_raster_tile_band_scatter_sort_multi: capacities")
     assert refused(sm(8, 2, dummy, dummy, dummy, 64, 64, caps, dummy, dummy, dummy, None, 2400, None, dummy, None),
                    "adb_raster_tile_band_scatter_sort_multi: null pointer")
+    assert refused(sm(8, 2, dummy, dummy, dummy, 64, 64, caps, dummy, dummy, dummy, dummy, 2400, None, None, None),
+                   "adb_raster_tile_band_scatter_sort_multi: null pointer")                      # vals are required
     assert refused(sm(8, 2, dummy, dummy, dummy, 64, 64, caps, dummy, dummy, dummy, dummy, 2399, None, dummy, None),
                    "scratch too small", status=3)
     assert sm(0, 2, None, None, None, 64, 64, caps, None, None, None, None, 0, None, None, None) == 0    # N = 0: no launch
@@ -181,9 +188,14 @@ def test_inria_rectangle_through_the_single_view_entry_point(cuda):
     radii, splats, tpg = R.project(t["means"], t["quats"], t["scales"], t["opacities"], t["sh"], 3, V.to(cuda), K.to(cuda),
                                    P, W, H, 0.01, 0.01, 1e10, 0.0, legacy=True)
     kb, vb, ob, nb = R.intersect(radii, splats, tpg, W, H, cam_id=1, n_cams=2, legacy=True)
-    kr, vr, orr, nr = R.intersect(radii, splats, tpg, W, H, cam_id=1, n_cams=2, legacy=True, method="radix")
-    assert nb == nr > 0
-    assert torch.equal(kb, kr) and torch.equal(vb, vr) and torch.equal(ob, orr)
+    # CPU reference: the gsplat key layout and stable sort over the Inria rectangle; a Gaussian the projection gave no
+    # tiles (opacity below 1/255) emits no keys
+    r, sp, t = radii.cpu(), splats.cpu(), tpg.cpu()
+    rect = lambda i, tw, th: legacy_torch._rect(sp[:, 0:2], r[:, 0], i, tw, th) if t[i] > 0 else None
+    kr, vr, orr = raster_torch.isect_and_sort(r, sp[:, 0:2], sp[:, 11], W, H, cam_id=1, n_cams=2, rect_fn=rect)
+    assert nb == len(kr) > 0
+    assert torch.equal(kb.cpu(), kr) and torch.equal(vb.cpu(), vr)
+    assert torch.equal(ob.cpu(), torch.cat([orr, torch.tensor([nb], dtype=torch.int32)]))
 
 
 def _single_raw(rec, W, H, dev, capacity, tail=64):

@@ -43,13 +43,6 @@ def test_multi_entry_points_refuse_bad_arguments_before_touching_the_device():
     assert refused(sc(2, 64, 64, huge, dummy, dummy, None, None, None), "adb_raster_tile_scan_multi: capacities")
     assert refused(sc(2, 64, 64, caps, None, dummy, None, None, None), "adb_raster_tile_scan_multi: null pointer")
     assert refused(sc(2, 64, 64, caps, dummy, None, None, None, None), "adb_raster_tile_scan_multi: null pointer")  # no output
-    ss = L.adb_raster_tile_scatter_sort_multi
-    assert refused(ss(8, 0, dummy, dummy, dummy, 64, 64, caps, dummy, dummy, dummy, None, dummy, None),
-                   "adb_raster_tile_scatter_sort_multi")
-    assert refused(ss(8, 2, dummy, dummy, dummy, 64, 64, huge, dummy, dummy, dummy, None, dummy, None),
-                   "adb_raster_tile_scatter_sort_multi: capacities")
-    assert refused(ss(8, 2, dummy, dummy, dummy, 64, 64, caps, dummy, dummy, dummy, None, None, None),
-                   "adb_raster_tile_scatter_sort_multi: null pointer")                                  # vals are required
     bf, bb = L.adb_raster_blend_fwd_multi, L.adb_raster_blend_bwd_multi
     assert refused(bf(8, 0, 64, 64, dummy, dummy, dummy, dummy, dummy, dummy, None, None), "adb_raster_blend_fwd_multi")
     assert refused(bf(8, 2, 64, 64, dummy, dummy, dummy, None, dummy, dummy, None, None), "adb_raster_blend_fwd_multi: null pointer")

@@ -1,12 +1,10 @@
-"""Scatter and sort of the multi-view tile intersection, timed apart, on the bench scene (1M Gaussians, 1920x1080, views
-0..7, the bench's seeds, capacities from MultiViewStep.calibrate).
+"""Band scatter and sort of the multi-view tile intersection (adb_raster_tile_band_scatter_sort_multi), timed apart, on the
+bench scene (1M Gaussians, 1920x1080, views 0..7, the bench's seeds, capacities from MultiViewStep.calibrate).
 
 Each timed launch is preceded, untimed, by what the step runs before it: counters zeroed, adb_raster_project_fwd_multi,
-adb_raster_tile_scan_multi.  For every scatter-sort entry point the library exports (the per-intersection scatter and,
-where present, the band scatter) it reports:
+adb_raster_tile_scan_multi.  It reports:
   * CUDA events around the whole entry point, per launch (--launches launches, after --warmup);
-  * the device time of each kernel inside it, from torch.profiler (CUDA activities, a separate run of --launches launches);
-  * whether vals and offsets equal the first entry point's, bit for bit.
+  * the device time of each kernel inside it, from torch.profiler (CUDA activities, a separate run of --launches launches).
 Prints one JSON line with the card's name and power limit read in the same process."""
 import argparse
 import ctypes as C
@@ -68,15 +66,13 @@ def main():
 
     args_in = lambda: (N, VIEWS, _lib.ptr(eng.radii), _lib.ptr(eng.splats), _lib.ptr(eng.tpg), W, H, caps,  # noqa: E731
                        _lib.ptr(eng.counts), _lib.ptr(offsets), _lib.ptr(packed))
-    paths = {"scatter": lambda: _lib.call("adb_raster_tile_scatter_sort_multi", *args_in(), None, _lib.ptr(vals), st())}
-    if "adb_raster_tile_band_scatter_sort_multi" in _lib._SIGS:
-        nb = C.c_size_t(0)
-        _lib.call("adb_raster_tile_band_scratch_bytes", total, C.byref(nb))
-        scratch = torch.empty(nb.value, dtype=torch.uint8, device=dev)
-        paths["band"] = lambda: _lib.call("adb_raster_tile_band_scatter_sort_multi", *args_in(), _lib.ptr(scratch),
-                                          scratch.numel(), None, _lib.ptr(vals), st())
+    nb = C.c_size_t(0)
+    _lib.call("adb_raster_tile_band_scratch_bytes", total, C.byref(nb))
+    scratch = torch.empty(nb.value, dtype=torch.uint8, device=dev)
+    paths = {"band": lambda: _lib.call("adb_raster_tile_band_scatter_sort_multi", *args_in(), _lib.ptr(scratch),
+                                       scratch.numel(), None, _lib.ptr(vals), st())}
 
-    res, first = {}, None
+    res = {}
     for name, fn in paths.items():
         for _ in range(args.warmup):
             prepare()
@@ -91,10 +87,6 @@ def main():
             b.record()
             torch.cuda.synchronize()
             ms.append(a.elapsed_time(b))
-        out = (vals.clone(), offsets.clone())
-        if first is None:
-            first = out
-        same = bool(torch.equal(out[0], first[0]) and torch.equal(out[1], first[1]))
         with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
             for _ in range(args.launches):
                 prepare()
@@ -106,7 +98,7 @@ def main():
                 short = re.search(r"(\w+_kernel)", ev.key).group(1)
                 kernels[short] = round(ev.device_time_total / 1e3 / args.launches, 4)     # ms per launch
         res[name] = {"ms_per_launch_median": round(statistics.median(ms), 4), "ms_min": round(min(ms), 4),
-                     "ms_max": round(max(ms), 4), "kernel_ms_per_launch": kernels, "vals_offsets_equal_first": same}
+                     "ms_max": round(max(ms), 4), "kernel_ms_per_launch": kernels}
     print(json.dumps({"label": args.label, "launches": args.launches, "n_isect": n_isect, "capacity": eng.capacity,
                       "paths": res, "device": torch.cuda.get_device_name(dev), "power_limit_w": power_limit_w()}),
           flush=True)

@@ -1,5 +1,5 @@
 """Per-stage live timing (CUDA events on the launching stream) of the rasterizer step at the bench workload, without the
-e2e / MASt3R / CPU legs.  ADB_ISECT=radix|bucket and ADB_BWD_SLOTS=16|32 select the A/B variants."""
+e2e / MASt3R / CPU legs.  ADB_BWD_SLOTS=16|32 selects the A/B variant."""
 import json
 import os
 import sys
@@ -57,6 +57,6 @@ for _ in range(steps):
 torch.cuda.synchronize()
 tot = _lib.TIMER.totals_ms()
 _lib.TIMER = None
-print(json.dumps({"isect": os.environ.get("ADB_ISECT", "bucket"), "bwd_slots": os.environ.get("ADB_BWD_SLOTS", "16"),
+print(json.dumps({"bwd_slots": os.environ.get("ADB_BWD_SLOTS", "16"),
                   "N": N, "W": W, "H": H, "ms_per_step": ms, "n_isect": info["n_isect"],
                   "stage_ms": {k.replace("adb_raster_", ""): round(v[0] / v[1], 4) for k, v in tot.items()}}))
