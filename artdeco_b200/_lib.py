@@ -78,7 +78,6 @@ LAUNCHES = {
     "adb_raster_blend_bwd": 1, "adb_raster_project_bwd": 1,
     "adb_raster_project_fwd_legacy": 1, "adb_raster_blend_fwd_legacy": 1,
     "adb_raster_blend_bwd_legacy": 1, "adb_raster_tile_count_scan": 2,
-    "adb_raster_blend_fwd_hits": 1, "adb_raster_blend_bwd_hits": 1,
     "adb_raster_project_bwd_multi": 1, "adb_raster_sh_bwd_multi": 1, "adb_raster_sh_dir_bwd_multi": 1,
     "adb_raster_sh_expand_multi": 1, "adb_raster_project_fwd_counts": 1, "adb_raster_tile_scan": 1,
     "adb_raster_project_fwd_multi": 1, "adb_raster_tile_scan_multi": 1,

@@ -21,7 +21,7 @@
 //        raw moments  sum_p vs(p) * {1, lx, ly, lx^2, lx ly, ly^2}   (vs = dL/dsigma, lx/ly = pixel offset in the block)
 //        feature grads sum_p fac(p) * v_out[p][0..3]                  (fac = alpha*T)
 //    i.e. a [slots x 32 pixels] x [32 x 10] product.  A lane therefore stores just (vs, fac) per evaluation (one STS.64)
-//    into a per-warp slot buffer; every S evaluations the warp transposes roles (lane = slot), streams the slot's row
+//    into a per-warp slot buffer; every SLOTS evaluations the warp transposes roles (lane = slot), streams the slot's row
 //    with LDS.128, applies the lane-constant integer weights as immediates (row sums first: 7.75 FMA per pixel
 //    instead of 10) and converts the block-origin moments to splat-centred ones once per (warp, splat):
 //        sum vs dx = ex S0 - Sx,  sum vs dx^2 = ex (ex S0 - 2 Sx) + Sxx, ...   (ex = mean_x - block origin)
@@ -29,7 +29,6 @@
 //    the nine moment/feature multiplies leave the per-pixel body as well;
 //  * results leave with three 128/64-bit vector REDs per (warp, splat) (red.global.add.v4.f32).
 #include "raster_common.cuh"
-#include <stdlib.h>
 
 namespace {
 
@@ -49,61 +48,6 @@ __device__ __forceinline__ float rcp_approx(float x) {
     float y;
     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
-}
-
-// ---- TMA (bulk async copy) staging: "stage Gaussian attributes into shared memory via TMA" (BASELINE north_star) ----------
-// Each thread issues ONE 48-byte cp.async.bulk (global -> shared, SASS UBLKCP) for the record of its list entry of the NEXT
-// batch; completion is tracked by an mbarrier per buffer (every thread arrives once; issuing threads add expect_tx 48).
-// The copy engine fills buffer (b+1)&1 while the warps evaluate batch b from buffer b&1, so the dependent-load latency of the
-// gather (vals[idx] -> splats[g]) no longer sits between two block barriers.  OPT-IN (ADB_BLEND_TMA=1): the blend kernels are
-// issue-bound with 3-4 resident CTAs per SM already hiding the gather latency, so the synchronous staging is the default.
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t.reg .pred P1;\n\t"
-        "WAIT_LOOP:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-        "@P1 bra DONE;\n\t"
-        "bra WAIT_LOOP;\n\t"
-        "DONE:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void bulk_copy_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-
-// Issues this thread's copy of record `g` into `rec` (48 B) or a plain arrival when the thread has no list entry.
-__device__ __forceinline__ void issue_record_copy(float4* rec, const float* __restrict__ splats, int g, bool have, uint64_t* bar) {
-    if (have) {
-        mbar_arrive_expect_tx(bar, ADB_SPLAT_STRIDE * 4);
-        bulk_copy_g2s(rec, splats + (size_t)g * ADB_SPLAT_STRIDE, ADB_SPLAT_STRIDE * 4, bar);
-    } else {
-        mbar_arrive(bar);
-    }
-}
-
-// In-place version of stage_record's pre-scaling for a record that arrived by bulk copy.
-template <bool LEGACY>
-__device__ __forceinline__ void prescale_record(float4* __restrict__ rec) {
-    float4 A = rec[0], B = rec[1];
-    A.z *= 0.5f * LOG2E;
-    A.w *= LOG2E;
-    B.x *= 0.5f * LOG2E;
-    B.z = (B.z - ADB_SIGMA_MARGIN) * LOG2E;
-    rec[0] = A;
-    rec[1] = B;
-    if (LEGACY) rec[2].w = 1.0f / rec[2].w;
 }
 
 // warp block geometry: warp w covers pixels x in [bx*16 + (w&1)*8, +8), y in [by*16 + (w>>1)*4, +4)
@@ -240,17 +184,15 @@ __device__ __forceinline__ int record_index(int v, int wrap) { return wrap ? v %
 // main_ids are [C,H,W,...] stacks.
 // LEGACY = Inria conventions (ADB_CONV_INRIA): alpha <= 0.99, stop when T(1-alpha) < 1e-4 (strict), 4th channel
 // accumulates 1/z, and main_ids gets the Gaussian with the largest blending weight alpha*T per pixel (-1: none).
-template <bool LEGACY, bool ASYNC>
+template <bool LEGACY>
 __global__ void __launch_bounds__(BLOCK, 4)
 blend_fwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* __restrict__ vals,
                  const int32_t* __restrict__ tile_offsets, int wrap,
                  float* __restrict__ colors, float* __restrict__ alphas, int32_t* __restrict__ last_ids,
                  int32_t* __restrict__ main_ids, unsigned char* __restrict__ hit_mask) {
     constexpr float MAXA = LEGACY ? ADB_MAX_ALPHA_INRIA : ADB_MAX_ALPHA;
-    constexpr int NBUF = ASYNC ? 2 : 1;
-    __shared__ __align__(16) float4 sRecBuf[NBUF][(BLOCK + 1) * 3];
+    __shared__ __align__(16) float4 sRec[(BLOCK + 1) * 3];
     __shared__ __align__(8) unsigned short sList[NWARP][LIST_STRIDE];
-    __shared__ __align__(8) uint64_t sBar[2];
     __shared__ unsigned sMask[BLOCK / 4];       // byte s = warp mask of slot s of the current batch (hit_mask != NULL)
 
     const int tw = (W + ADB_TILE - 1) / ADB_TILE;
@@ -278,23 +220,8 @@ blend_fwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
         }
     };
     int pending = -1;                            // batch whose masks are complete but not written yet (block-uniform)
-    if (tid == 0) {
-        write_dummy(sRecBuf[0] + DUMMY * 3);
-        if (ASYNC) {
-            write_dummy(sRecBuf[NBUF - 1] + DUMMY * 3);
-            mbar_init(&sBar[0], BLOCK);
-            mbar_init(&sBar[1], BLOCK);
-            fence_mbar_init();
-        }
-    }
+    if (tid == 0) write_dummy(sRec + DUMMY * 3);
     const int nb = (end - start + BLOCK - 1) / BLOCK;
-    if (ASYNC) {
-        __syncthreads();
-        if (nb > 0) {       // prologue: batch 0 -> buffer 0
-            const int idx0 = start + tid;
-            issue_record_copy(sRecBuf[0] + tid * 3, splats, idx0 < end ? record_index(vals[idx0], wrap) : 0, idx0 < end, &sBar[0]);
-        }
-    }
 
     float T = 1.0f;
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -307,21 +234,8 @@ blend_fwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
         if (hit_mask && pending >= 0) { flush_mask(pending); pending = -1; }
         const int bstart = start + b * BLOCK;
         const int idx = bstart + tid;
-        float4* sRec = sRecBuf[ASYNC ? (b & 1) : 0];
-        if (ASYNC) {
-            if (n_done >= BLOCK) { mbar_wait(&sBar[b & 1], (b >> 1) & 1); break; }   // drain the copy in flight, then leave
-            if (b + 1 < nb) {                            // prefetch batch b+1 into the buffer batch b-1 has just released
-                const int idx1 = idx + BLOCK;
-                fence_proxy_async();
-                issue_record_copy(sRecBuf[(b + 1) & 1] + tid * 3, splats, idx1 < end ? record_index(vals[idx1], wrap) : 0, idx1 < end,
-                                  &sBar[(b + 1) & 1]);
-            }
-            mbar_wait(&sBar[b & 1], (b >> 1) & 1);
-            if (idx < end) prescale_record<LEGACY>(sRec + tid * 3);
-        } else {
-            if (n_done >= BLOCK) break;
-            if (idx < end) stage_record<LEGACY>(sRec + tid * 3, splats, record_index(vals[idx], wrap));
-        }
+        if (n_done >= BLOCK) break;
+        if (idx < end) stage_record<LEGACY>(sRec + tid * 3, splats, record_index(vals[idx], wrap));
         __syncthreads();
         pending = b;
         const int bsize = min(BLOCK, end - bstart);
@@ -384,40 +298,35 @@ __device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
     asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
 
-// Backward shared-memory layout (dynamic): S = slots per warp in the deferred-reduction buffer (16 or 32).
-template <int S, bool ASYNC>
+// Slots per warp in the backward's deferred-reduction buffer: 32 would fit only 2 CTAs/SM.
+constexpr int SLOTS = 16;
+
+// Backward shared-memory layout (dynamic).
 struct BwdSmem {
-    static constexpr int NBUF = ASYNC ? 2 : 1;
     static constexpr int ROW4 = 17;                       // float4 per slot row: 32 x (vs, fac) + 1 pad -> conflict-free
-    static constexpr int REC_BYTES = (BLOCK + 1) * 3 * 16;
-    static constexpr int G_BYTES = (BLOCK + 4) * 4;
-    static constexpr int OFF_REC = 0;                     // float4 [NBUF][(BLOCK+1)*3]
-    static constexpr int OFF_G = OFF_REC + NBUF * REC_BYTES;                  // int [NBUF][BLOCK + 4]
-    static constexpr int OFF_BAR = OFF_G + NBUF * G_BYTES;                    // uint64 [2]
-    static constexpr int OFF_M = OFF_BAR + 16;                                // u8 [BLOCK]: the forward's warp masks of the batch
+    static constexpr int OFF_REC = 0;                                         // float4 [(BLOCK+1)*3]
+    static constexpr int OFF_G = OFF_REC + (BLOCK + 1) * 3 * 16;              // int [BLOCK + 4]
+    static constexpr int OFF_M = OFF_G + (BLOCK + 4) * 4;                     // u8 [BLOCK]: the forward's warp masks of the batch
     static constexpr int OFF_LIST = OFF_M + BLOCK;                            // u16 [NWARP][LIST_STRIDE]
     static constexpr int OFF_VO = OFF_LIST + NWARP * LIST_STRIDE * 2;         // float4 [NWARP][32]
-    static constexpr int OFF_V = OFF_VO + NWARP * 32 * 16;                    // float4 [NWARP][S*ROW4]
-    static constexpr int BYTES = OFF_V + NWARP * S * ROW4 * 16;
-    static_assert(OFF_G % 16 == 0 && OFF_BAR % 16 == 0 && OFF_LIST % 16 == 0 && OFF_VO % 16 == 0 && OFF_V % 16 == 0, "alignment");
+    static constexpr int OFF_V = OFF_VO + NWARP * 32 * 16;                    // float4 [NWARP][SLOTS*ROW4]
+    static constexpr int BYTES = OFF_V + NWARP * SLOTS * ROW4 * 16;
+    static_assert(OFF_G % 16 == 0 && OFF_LIST % 16 == 0 && OFF_VO % 16 == 0 && OFF_V % 16 == 0, "alignment");
 };
 
-template <bool LEGACY, int S, int OCC, bool ASYNC>
-__global__ void __launch_bounds__(BLOCK, OCC)
+// The default build fits 4 CTAs/SM (64 registers); the legacy build is bounded for 3.
+template <bool LEGACY>
+__global__ void __launch_bounds__(BLOCK, LEGACY ? 3 : 4)
 blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* __restrict__ vals,
                  const int32_t* __restrict__ tile_offsets, int wrap,
                  const float* __restrict__ alphas, const int32_t* __restrict__ last_ids,
                  const float* __restrict__ v_colors, const float* __restrict__ v_alphas,
                  float* __restrict__ v_splats, const unsigned char* __restrict__ hit_mask) {
     constexpr float MAXA = LEGACY ? ADB_MAX_ALPHA_INRIA : ADB_MAX_ALPHA;
-    using L = BwdSmem<S, ASYNC>;
-    constexpr int HALVES = 32 / S;          // lanes per slot in the reduction phase
-    constexpr int ROWS = 4 / HALVES;        // pixel rows (of 8) each reduction lane walks
-    static_assert(S == 16 || S == 32, "S");
+    using L = BwdSmem;
     extern __shared__ __align__(16) unsigned char smem[];
     float4* sRec = reinterpret_cast<float4*>(smem + L::OFF_REC);
     int* sG = reinterpret_cast<int*>(smem + L::OFF_G);
-    uint64_t* sBar = reinterpret_cast<uint64_t*>(smem + L::OFF_BAR);
     unsigned char* sM = smem + L::OFF_M;
 
     const int tw = (W + ADB_TILE - 1) / ADB_TILE;
@@ -425,7 +334,7 @@ blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     unsigned short* list = reinterpret_cast<unsigned short*>(smem + L::OFF_LIST) + warp * LIST_STRIDE;
     float4* sVo = reinterpret_cast<float4*>(smem + L::OFF_VO) + warp * 32;
-    float4* sV = reinterpret_cast<float4*>(smem + L::OFF_V) + warp * S * L::ROW4;
+    float4* sV = reinterpret_cast<float4*>(smem + L::OFF_V) + warp * SLOTS * L::ROW4;
     const int x0 = blockIdx.x * ADB_TILE + (warp & 1) * 8, y0 = blockIdx.y * ADB_TILE + (warp >> 1) * 4;
     const int j = x0 + (lane & 7), i = y0 + (lane >> 3);
     const bool inside = (i < H && j < W);
@@ -448,55 +357,25 @@ blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
     if (tid == 0) {
         write_dummy(sRec + DUMMY * 3);
         sG[DUMMY] = 0;
-        if (ASYNC) {
-            write_dummy(reinterpret_cast<float4*>(smem + L::OFF_REC + L::REC_BYTES) + DUMMY * 3);
-            reinterpret_cast<int*>(smem + L::OFF_G + L::G_BYTES)[DUMMY] = 0;
-            mbar_init(&sBar[0], BLOCK);
-            mbar_init(&sBar[1], BLOCK);
-            fence_mbar_init();
-        }
     }
 
     int warp_bin_final = bin_final;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) warp_bin_final = max(warp_bin_final, __shfl_xor_sync(FULL, warp_bin_final, o));
 
-    // reduction-phase role of this lane: slot r_slot, pixel rows [r_half*ROWS, +ROWS) of the warp's 8x4 block
-    const int r_slot = lane & (S - 1), r_half = lane / S;
-    const float4* r_row = sV + r_slot * L::ROW4 + r_half * (ROWS * 4);
-    const float4* r_vo = sVo + r_half * (ROWS * 8);
+    // reduction-phase role of this lane: slot r_slot, pixel rows [2*r_half, +2) of the warp's 8x4 block
+    const int r_slot = lane & (SLOTS - 1), r_half = lane / SLOTS;
+    const float4* r_row = sV + r_slot * L::ROW4 + r_half * 8;
+    const float4* r_vo = sVo + r_half * 16;
     float2* my_cell = reinterpret_cast<float2*>(sV) + lane;          // + slot * ROW4 * 2 (float2 units)
 
     const int nb = (end - start + BLOCK - 1) / BLOCK;
-    if (ASYNC) {
-        __syncthreads();
-        const int idx0 = end - 1 - tid;                      // prologue: batch 0 -> buffer 0
-        const int g0 = idx0 >= start ? record_index(vals[idx0], wrap) : 0;
-        if (idx0 >= start) sG[tid] = g0;
-        issue_record_copy(sRec + tid * 3, splats, g0, idx0 >= start, &sBar[0]);
-    }
-    float4* const sRec0 = sRec;
-    int* const sG0 = sG;
     for (int b = 0; b < nb; ++b) {
         __syncthreads();  // previous batch fully consumed
         const int batch_end = end - 1 - b * BLOCK;           // smem slot t <-> sorted index batch_end - t (back to front)
         const int bsize = min(BLOCK, batch_end + 1 - start);
         const int idx = batch_end - tid;
-        if (ASYNC) {
-            sRec = reinterpret_cast<float4*>(reinterpret_cast<unsigned char*>(sRec0) + (b & 1) * L::REC_BYTES);
-            sG = reinterpret_cast<int*>(reinterpret_cast<unsigned char*>(sG0) + (b & 1) * L::G_BYTES);
-            if (b + 1 < nb) {                                // prefetch batch b+1 into the buffer batch b-1 has just released
-                const int nbuf = (b + 1) & 1;
-                const int idx1 = idx - BLOCK;
-                const int g1 = idx1 >= start ? record_index(vals[idx1], wrap) : 0;
-                if (idx1 >= start) reinterpret_cast<int*>(reinterpret_cast<unsigned char*>(sG0) + nbuf * L::G_BYTES)[tid] = g1;
-                fence_proxy_async();
-                issue_record_copy(reinterpret_cast<float4*>(reinterpret_cast<unsigned char*>(sRec0) + nbuf * L::REC_BYTES) + tid * 3,
-                                  splats, g1, idx1 >= start, &sBar[nbuf]);
-            }
-            mbar_wait(&sBar[b & 1], (b >> 1) & 1);
-            if (idx >= start) prescale_record<LEGACY>(sRec + tid * 3);
-        } else if (idx >= start) {
+        if (idx >= start) {
             const int g = record_index(vals[idx], wrap);
             sG[tid] = g;
             stage_record<LEGACY>(sRec + tid * 3, splats, g);
@@ -509,8 +388,8 @@ blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
         const int nhit = hit_mask ? build_hit_list_from_mask(sM, list, bsize, limit, warp, lane)
                                   : build_hit_list(sRec, list, bsize, limit, rect, lane);
         const int tmin = inside ? batch_end - bin_final : (1 << 30);   // lane-valid iff t >= tmin
-        for (int g0 = 0; g0 < nhit; g0 += S) {
-            const int ng = min(S, nhit - g0);
+        for (int g0 = 0; g0 < nhit; g0 += SLOTS) {
+            const int ng = min(SLOTS, nhit - g0);
             const int nq = (ng + 3) >> 2;
             for (int q = 0; q < nq; ++q) {
                 const uint2 pk = *reinterpret_cast<const uint2*>(list + g0 + 4 * q);
@@ -544,7 +423,7 @@ blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
             // ---- deferred reduction: lane = (slot, pixel-row group) ----
             float S0 = 0.f, Sx = 0.f, Sy = 0.f, Sxx = 0.f, Sxy = 0.f, Syy = 0.f, c0 = 0.f, c1 = 0.f, c2 = 0.f, c3 = 0.f;
 #pragma unroll
-            for (int r = 0; r < ROWS; ++r) {
+            for (int r = 0; r < 2; ++r) {
                 float R0 = 0.f, R1 = 0.f, R2 = 0.f;
 #pragma unroll
                 for (int x = 0; x < 8; x += 2) {
@@ -559,17 +438,15 @@ blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
                     R2 = fmaf(v.z, (float)((x + 1) * (x + 1)), R2);
                     c0 = fmaf(v.w, w1.x, c0); c1 = fmaf(v.w, w1.y, c1); c2 = fmaf(v.w, w1.z, c2); c3 = fmaf(v.w, w1.w, c3);
                 }
-                const float ly = (float)(r_half * ROWS + r);
+                const float ly = (float)(r_half * 2 + r);
                 S0 += R0; Sx += R1; Sxx += R2;
                 Sy = fmaf(ly, R0, Sy); Sxy = fmaf(ly, R1, Sxy); Syy = fmaf(ly * ly, R0, Syy);
             }
-            if (HALVES == 2) {
-                S0 += __shfl_xor_sync(FULL, S0, 16); Sx += __shfl_xor_sync(FULL, Sx, 16);
-                Sy += __shfl_xor_sync(FULL, Sy, 16); Sxx += __shfl_xor_sync(FULL, Sxx, 16);
-                Sxy += __shfl_xor_sync(FULL, Sxy, 16); Syy += __shfl_xor_sync(FULL, Syy, 16);
-                c0 += __shfl_xor_sync(FULL, c0, 16); c1 += __shfl_xor_sync(FULL, c1, 16);
-                c2 += __shfl_xor_sync(FULL, c2, 16); c3 += __shfl_xor_sync(FULL, c3, 16);
-            }
+            S0 += __shfl_xor_sync(FULL, S0, 16); Sx += __shfl_xor_sync(FULL, Sx, 16);
+            Sy += __shfl_xor_sync(FULL, Sy, 16); Sxx += __shfl_xor_sync(FULL, Sxx, 16);
+            Sxy += __shfl_xor_sync(FULL, Sxy, 16); Syy += __shfl_xor_sync(FULL, Syy, 16);
+            c0 += __shfl_xor_sync(FULL, c0, 16); c1 += __shfl_xor_sync(FULL, c1, 16);
+            c2 += __shfl_xor_sync(FULL, c2, 16); c3 += __shfl_xor_sync(FULL, c3, 16);
             if (r_slot < ng) {
                 const int t = list[g0 + r_slot];
                 const float4 A = sRec[t * 3];
@@ -582,11 +459,6 @@ blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
                         const float Mxx = fmaf(ex, fmaf(ex, S0, -2.f * Sx), Sxx);
                         const float Mxy = fmaf(ex, My, fmaf(-ey, Sx, Sxy));
                         red_add_v4(dst, Mx, My, Mxx, Mxy);
-                    }
-                    if (HALVES == 1) {
-                        const float Myy = fmaf(ey, fmaf(ey, S0, -2.f * Sy), Syy);
-                        if (Myy != 0.f || S0 != 0.f || c0 != 0.f || c1 != 0.f) red_add_v4(dst + 4, Myy, S0, c0, c1);
-                        if (c2 != 0.f || c3 != 0.f) red_add_v2(dst + 8, c2, c3);
                     }
                 } else {
                     const float Myy = fmaf(ey, fmaf(ey, S0, -2.f * Sy), Syy);
@@ -605,22 +477,16 @@ blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
 static int blend_fwd_impl(bool legacy, int C, int W, int H, int wrap, const float* splats, const int32_t* vals_sorted,
                           const int32_t* tile_offsets, float* colors, float* alphas, int32_t* last_ids,
                           int32_t* main_ids, unsigned char* hit_mask, cudaStream_t stream) {
-    // records are read as float4 (or by 48-byte bulk copies) and colours stored as float4: a misaligned view would fault
+    // records are read and colours stored as float4: a misaligned view would fault
     ADB_REQUIRE((((uintptr_t)splats | (uintptr_t)colors) % 16) == 0,
                 "adb_raster_blend_fwd: splats and colors must be 16-byte aligned");
     dim3 grid(adb_cdiv(W, ADB_TILE), adb_cdiv(H, ADB_TILE), C);
-    // ADB_BLEND_TMA=1: double-buffered cp.async.bulk (TMA) staging.  Default: synchronous LDG staging (the kernel is
-    // issue-bound with 4 CTAs/SM hiding the gather latency, so the extra prescale pass and mbarrier waits buy nothing).
-    static const int tma = getenv("ADB_BLEND_TMA") ? atoi(getenv("ADB_BLEND_TMA")) : 0;
     if (legacy)
-        blend_fwd_kernel<true, false><<<grid, BLOCK, 0, stream>>>(W, H, splats, vals_sorted, tile_offsets, wrap,
-                                                                 colors, alphas, last_ids, main_ids, hit_mask);
-    else if (tma)
-        blend_fwd_kernel<false, true><<<grid, BLOCK, 0, stream>>>(W, H, splats, vals_sorted, tile_offsets, wrap,
-                                                                 colors, alphas, last_ids, nullptr, hit_mask);
+        blend_fwd_kernel<true><<<grid, BLOCK, 0, stream>>>(W, H, splats, vals_sorted, tile_offsets, wrap,
+                                                           colors, alphas, last_ids, main_ids, hit_mask);
     else
-        blend_fwd_kernel<false, false><<<grid, BLOCK, 0, stream>>>(W, H, splats, vals_sorted, tile_offsets, wrap,
-                                                                  colors, alphas, last_ids, nullptr, hit_mask);
+        blend_fwd_kernel<false><<<grid, BLOCK, 0, stream>>>(W, H, splats, vals_sorted, tile_offsets, wrap,
+                                                            colors, alphas, last_ids, nullptr, hit_mask);
     ADB_CHECK_LAUNCH("blend_fwd_kernel");
     return ADB_OK;
 }
@@ -635,27 +501,19 @@ static int blend_fwd_single(bool legacy, int W, int H, int n_per_cam, const floa
 }
 
 // `vals` are the sorted values (cam*N + gaussian); n_per_cam = N.  colors [H,W,4], alphas [H,W], last_ids [H,W].
+// hit_mask (may be NULL): hit_mask[k] (one byte per sorted intersection, k as in vals_sorted) receives the warps of entry k's
+// tile whose 8x4 pixel block the splat can reach — the culling decisions of this pass, which adb_raster_blend_bwd reuses.
+// Entries behind the point where a whole tile saturated are left unwritten (the backward never looks at them).
 ADB_API int adb_raster_blend_fwd(int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
                                  const int32_t* tile_offsets, float* colors, float* alphas, int32_t* last_ids,
-                                 cudaStream_t stream) {
-    return blend_fwd_single(false, W, H, n_per_cam, splats, vals_sorted, tile_offsets, colors, alphas, last_ids, nullptr,
-                            nullptr, stream);
-}
-
-// Same, and hit_mask[k] (one byte per sorted intersection, k as in vals_sorted) receives the warps of entry k's tile whose 8x4
-// pixel block the splat can reach — the culling decisions of this pass, which adb_raster_blend_bwd_hits reuses.  Entries behind
-// the point where a whole tile saturated are left unwritten (the backward never looks at them).
-ADB_API int adb_raster_blend_fwd_hits(int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
-                                      const int32_t* tile_offsets, float* colors, float* alphas, int32_t* last_ids,
-                                      unsigned char* hit_mask, cudaStream_t stream) {
-    ADB_REQUIRE(hit_mask, "adb_raster_blend_fwd_hits: null hit_mask");
+                                 unsigned char* hit_mask, cudaStream_t stream) {
     return blend_fwd_single(false, W, H, n_per_cam, splats, vals_sorted, tile_offsets, colors, alphas, last_ids, nullptr,
                             hit_mask, stream);
 }
 
 // C views in one launch (the multi-view batch): splats [C,N,12] indexed by vals_sorted (= c*N + gaussian) directly,
 // tile_offsets [C,T+1] absolute (adb_raster_tile_scan_multi), colors [C,H,W,4], alphas / last_ids [C,H,W]; hit_mask (may be
-// NULL) indexed like vals_sorted.  Per view the result of adb_raster_blend_fwd_hits on that view's records, bit for bit;
+// NULL) indexed like vals_sorted.  Per view the result of adb_raster_blend_fwd on that view's records, bit for bit;
 // last_ids are absolute sorted indices.  N = 0 (no Gaussians: every tile is empty) writes empty images; splats may be NULL.
 ADB_API int adb_raster_blend_fwd_multi(int N, int C, int W, int H, const float* splats, const int32_t* vals_sorted,
                                        const int32_t* tile_offsets, float* colors, float* alphas, int32_t* last_ids,
@@ -675,22 +533,6 @@ ADB_API int adb_raster_blend_fwd_legacy(int W, int H, int n_per_cam, const float
                             nullptr, stream);
 }
 
-template <bool LEGACY, int S, int OCC, bool ASYNC>
-static int launch_bwd(dim3 grid, int W, int H, int wrap, const float* splats, const int32_t* vals_sorted,
-                      const int32_t* tile_offsets, const float* alphas, const int32_t* last_ids, const float* v_colors,
-                      const float* v_alphas, float* v_splats, const unsigned char* hit_mask, cudaStream_t stream) {
-    static AdbDeviceOnce once;
-    const int rc = once.ensure([]() -> int {
-        ADB_CUDA(cudaFuncSetAttribute(blend_bwd_kernel<LEGACY, S, OCC, ASYNC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      BwdSmem<S, ASYNC>::BYTES));
-        return ADB_OK;
-    });
-    if (rc != ADB_OK) return rc;
-    blend_bwd_kernel<LEGACY, S, OCC, ASYNC><<<grid, BLOCK, BwdSmem<S, ASYNC>::BYTES, stream>>>(
-        W, H, splats, vals_sorted, tile_offsets, wrap, alphas, last_ids, v_colors, v_alphas, v_splats, hit_mask);
-    return ADB_OK;
-}
-
 // C views (gridDim.z); wrap: see record_index.
 static int blend_bwd_impl(bool legacy, int C, int W, int H, int wrap, const float* splats, const int32_t* vals_sorted,
                           const int32_t* tile_offsets, const float* alphas, const int32_t* last_ids,
@@ -700,22 +542,19 @@ static int blend_bwd_impl(bool legacy, int C, int W, int H, int wrap, const floa
     ADB_REQUIRE((((uintptr_t)splats | (uintptr_t)v_colors | (uintptr_t)v_splats) % 16) == 0,
                 "adb_raster_blend_bwd: splats, v_colors and v_splats must be 16-byte aligned");
     dim3 grid(adb_cdiv(W, ADB_TILE), adb_cdiv(H, ADB_TILE), C);
-    // A/B switches: ADB_BWD_SLOTS=32 -> 32-slot deferred-reduction buffer (2 CTAs/SM);
-    // ADB_BWD_OCC=3 -> 79 registers, 3 CTAs/SM instead of the default 64 registers, 4 CTAs/SM.
-    static const int slots = getenv("ADB_BWD_SLOTS") ? atoi(getenv("ADB_BWD_SLOTS")) : 16;
-    static const int occ = getenv("ADB_BWD_OCC") ? atoi(getenv("ADB_BWD_OCC")) : 4;
-    int rc;
-#define ADB_BWD_ARGS grid, W, H, wrap, splats, vals_sorted, tile_offsets, alphas, last_ids, v_colors, v_alphas, v_splats, hit_mask, stream
-    // ADB_BLEND_TMA=1: double-buffered cp.async.bulk staging (+13 KB of shared memory: 3 CTAs/SM instead of 4); opt-in for
-    // the same reason as the forward kernel.
-    static const int tma = getenv("ADB_BLEND_TMA") ? atoi(getenv("ADB_BLEND_TMA")) : 0;
-    if (legacy) rc = launch_bwd<true, 16, 3, false>(ADB_BWD_ARGS);
-    else if (slots == 32) rc = launch_bwd<false, 32, 2, false>(ADB_BWD_ARGS);
-    else if (tma) rc = launch_bwd<false, 16, 3, true>(ADB_BWD_ARGS);
-    else if (occ == 4) rc = launch_bwd<false, 16, 4, false>(ADB_BWD_ARGS);
-    else rc = launch_bwd<false, 16, 3, false>(ADB_BWD_ARGS);
-#undef ADB_BWD_ARGS
+    static AdbDeviceOnce once;
+    const int rc = once.ensure([]() -> int {
+        ADB_CUDA(cudaFuncSetAttribute(blend_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem::BYTES));
+        ADB_CUDA(cudaFuncSetAttribute(blend_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem::BYTES));
+        return ADB_OK;
+    });
     if (rc != ADB_OK) return rc;
+    if (legacy)
+        blend_bwd_kernel<true><<<grid, BLOCK, BwdSmem::BYTES, stream>>>(W, H, splats, vals_sorted, tile_offsets, wrap, alphas,
+                                                                        last_ids, v_colors, v_alphas, v_splats, hit_mask);
+    else
+        blend_bwd_kernel<false><<<grid, BLOCK, BwdSmem::BYTES, stream>>>(W, H, splats, vals_sorted, tile_offsets, wrap, alphas,
+                                                                         last_ids, v_colors, v_alphas, v_splats, hit_mask);
     ADB_CHECK_LAUNCH("blend_bwd_kernel");
     return ADB_OK;
 }
@@ -732,22 +571,13 @@ static int blend_bwd_single(bool legacy, int W, int H, int n_per_cam, const floa
                           v_splats, hit_mask, stream);
 }
 
-// v_splats [N,12] must be zeroed by the caller; gradients are accumulated into it.
+// v_splats [N,12] must be zeroed by the caller; gradients are accumulated into it.  hit_mask (may be NULL): the forward's
+// culling decisions (adb_raster_blend_fwd of the SAME splats / vals_sorted / tile_offsets); the per-warp hit lists then come
+// from it instead of repeating the box and ellipse tests.  Identical gradients either way.
 ADB_API int adb_raster_blend_bwd(int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
                                  const int32_t* tile_offsets, const float* alphas, const int32_t* last_ids,
                                  const float* v_colors, const float* v_alphas, float* v_splats,
-                                 cudaStream_t stream) {
-    return blend_bwd_single(false, W, H, n_per_cam, splats, vals_sorted, tile_offsets, alphas, last_ids, v_colors,
-                            v_alphas, v_splats, nullptr, stream);
-}
-
-// Same with the forward's culling decisions (adb_raster_blend_fwd_hits of the SAME splats / vals_sorted / tile_offsets): the
-// per-warp hit lists come from hit_mask instead of repeating the box and ellipse tests.  Identical gradients.
-ADB_API int adb_raster_blend_bwd_hits(int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
-                                      const int32_t* tile_offsets, const float* alphas, const int32_t* last_ids,
-                                      const float* v_colors, const float* v_alphas, float* v_splats,
-                                      const unsigned char* hit_mask, cudaStream_t stream) {
-    ADB_REQUIRE(hit_mask, "adb_raster_blend_bwd_hits: null hit_mask");
+                                 const unsigned char* hit_mask, cudaStream_t stream) {
     return blend_bwd_single(false, W, H, n_per_cam, splats, vals_sorted, tile_offsets, alphas, last_ids, v_colors,
                             v_alphas, v_splats, hit_mask, stream);
 }

@@ -10,7 +10,6 @@ All compute goes through the C ABI (adb_raster_*); PyTorch only owns memory, str
 from __future__ import annotations
 
 import ctypes as C
-import os
 from typing import Optional
 
 import torch
@@ -27,8 +26,8 @@ _lib.register("adb_raster_tile_count_scan", [i32, vp, vp, vp, i32, i32, i32, i64
 _lib.register("adb_raster_tile_band_scratch_bytes", [i64, C.POINTER(C.c_size_t)])
 _lib.register("adb_raster_tile_band_scatter_sort", [i32, vp, vp, vp, i32, i32, i32, i32, i32, i64, vp, vp, vp, vp,
                                                     C.c_size_t, vp, vp, vp])
-_lib.register("adb_raster_blend_fwd", [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp])
-_lib.register("adb_raster_blend_bwd", [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp])
+_lib.register("adb_raster_blend_fwd", [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp])
+_lib.register("adb_raster_blend_bwd", [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp])
 _lib.register("adb_raster_project_bwd", [i32, vp, vp, vp, vp, i32, vp, vp, vp, i32, i32, f32, f32, f32, f32,
                                          vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp])
 
@@ -39,8 +38,6 @@ _lib.register("adb_raster_sh_expand_multi", [i32, i32, vp, i32, vp, vp, vp, vp])
 
 _lib.register("adb_raster_project_fwd_legacy", [i32, vp, vp, vp, vp, vp, i32, vp, vp, vp, i32, i32, f32, f32, f32,
                                                 vp, vp, vp, vp])
-_lib.register("adb_raster_blend_fwd_hits", [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp])
-_lib.register("adb_raster_blend_bwd_hits", [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp])
 _lib.register("adb_raster_blend_fwd_legacy", [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp])
 _lib.register("adb_raster_blend_bwd_legacy", [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp])
 
@@ -287,9 +284,7 @@ def intersect(radii, splats, tpg, W, H, cam_id=0, n_cams=1, legacy=False, capaci
 def new_hit_mask(vals: torch.Tensor):
     """One byte per sorted intersection for ``blend_forward(hits=)`` / ``blend_backward(hits=)``: the forward records which
     warps' pixel blocks each (tile, splat) entry can reach and the backward reuses those culling decisions instead of repeating
-    the tests.  ``ADB_BLEND_HITS=0`` returns None (both kernels then cull on their own)."""
-    if os.environ.get("ADB_BLEND_HITS", "1") == "0":
-        return None
+    the tests."""
     return torch.empty(max(1, vals.numel()), dtype=torch.uint8, device=vals.device)
 
 
@@ -313,11 +308,8 @@ def blend_forward(W, H, N, splats, vals, offsets, legacy=False, out=None, hits=N
     if hits is not None:
         if hits.dtype != torch.uint8 or hits.numel() < vals.numel() or hits.device != splats.device:
             raise ValueError("blend_forward: hits must be a uint8 tensor with one byte per intersection (new_hit_mask)")
-        _lib.call("adb_raster_blend_fwd_hits", W, H, N, _lib.ptr(splats), _lib.ptr(vals) if vals.numel() else None,
-                  _lib.ptr(offsets), _lib.ptr(colors), _lib.ptr(alphas), _lib.ptr(last_ids), _lib.ptr(hits), _lib.stream())
-        return colors, alphas, last_ids
     _lib.call("adb_raster_blend_fwd", W, H, N, _lib.ptr(splats), _lib.ptr(vals) if vals.numel() else None,
-              _lib.ptr(offsets), _lib.ptr(colors), _lib.ptr(alphas), _lib.ptr(last_ids), _lib.stream())
+              _lib.ptr(offsets), _lib.ptr(colors), _lib.ptr(alphas), _lib.ptr(last_ids), _lib.ptr(hits), _lib.stream())
     return colors, alphas, last_ids
 
 
@@ -325,16 +317,17 @@ def blend_backward(W, H, N, splats, vals, offsets, alphas, last_ids, v_colors, v
     """``out``: optional ZEROED [N,12] accumulator (a slice of the per-camera stack in the multi-view path).
     ``hits``: the mask ``blend_forward(hits=)`` filled for the SAME splats / vals / offsets."""
     v_splats = out if out is not None else torch.zeros(N, SPLAT_STRIDE, dtype=torch.float32, device=splats.device)
-    if hits is not None and not legacy:
+    if legacy:
+        _lib.call("adb_raster_blend_bwd_legacy", W, H, N, _lib.ptr(splats), _lib.ptr(vals) if vals.numel() else None,
+                  _lib.ptr(offsets), _lib.ptr(alphas), _lib.ptr(last_ids), _lib.ptr(v_colors), _lib.ptr(v_alphas),
+                  _lib.ptr(v_splats), _lib.stream())
+        return v_splats
+    if hits is not None:
         if hits.dtype != torch.uint8 or hits.numel() < vals.numel() or hits.device != splats.device:
             raise ValueError("blend_backward: hits must be the uint8 mask blend_forward filled for these intersections")
-        _lib.call("adb_raster_blend_bwd_hits", W, H, N, _lib.ptr(splats), _lib.ptr(vals) if vals.numel() else None,
-                  _lib.ptr(offsets), _lib.ptr(alphas), _lib.ptr(last_ids), _lib.ptr(v_colors), _lib.ptr(v_alphas),
-                  _lib.ptr(v_splats), _lib.ptr(hits), _lib.stream())
-        return v_splats
-    _lib.call("adb_raster_blend_bwd_legacy" if legacy else "adb_raster_blend_bwd", W, H, N, _lib.ptr(splats), _lib.ptr(vals) if vals.numel() else None,
+    _lib.call("adb_raster_blend_bwd", W, H, N, _lib.ptr(splats), _lib.ptr(vals) if vals.numel() else None,
               _lib.ptr(offsets), _lib.ptr(alphas), _lib.ptr(last_ids), _lib.ptr(v_colors), _lib.ptr(v_alphas),
-              _lib.ptr(v_splats), _lib.stream())
+              _lib.ptr(v_splats), _lib.ptr(hits), _lib.stream())
     return v_splats
 
 

@@ -260,26 +260,21 @@ int adb_raster_tile_band_scatter_sort_multi(int N, int C, const int32_t* radii, 
                                             const long long* capacities /*HOST [C]*/, int32_t* tile_counts,
                                             const int32_t* tile_offsets, void* packed, void* scratch, size_t scratch_bytes,
                                             int64_t* keys, int32_t* vals, adb_stream_t stream);
+/* Single-view blend pair.  hit_mask (may be NULL) shares the culling decisions: a non-NULL hit_mask makes the forward fill
+ * one byte per sorted intersection (index as in vals_sorted): bit w = the splat can reach the 8x4 pixel block of warp w of its
+ * tile (entries behind the point where a whole tile saturated are left unwritten).  Given that mask, the backward builds its
+ * per-warp hit lists from it instead of repeating the box and ellipse tests (same splats / vals_sorted / tile_offsets;
+ * identical gradients).  With NULL the forward writes no mask and the backward culls on its own. */
 int adb_raster_blend_fwd(int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
                          const int32_t* tile_offsets, float* colors /*[H,W,4]*/, float* alphas /*[H,W]*/,
-                         int32_t* last_ids /*[H,W]*/, adb_stream_t stream);
+                         int32_t* last_ids /*[H,W]*/, unsigned char* hit_mask /*may be NULL*/, adb_stream_t stream);
 int adb_raster_blend_bwd(int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
                          const int32_t* tile_offsets, const float* alphas, const int32_t* last_ids,
                          const float* v_colors, const float* v_alphas, float* v_splats /*[N,12] zeroed, +=*/,
-                         adb_stream_t stream);
-/* The same pair sharing the culling decisions: adb_raster_blend_fwd_hits also fills hit_mask — one byte per sorted intersection
- * (index as in vals_sorted): bit w = the splat can reach the 8x4 pixel block of warp w of its tile (entries behind the point
- * where a whole tile saturated are left unwritten) — and adb_raster_blend_bwd_hits builds its per-warp hit lists from it
- * instead of repeating the box and ellipse tests (same splats / vals_sorted / tile_offsets; identical gradients). */
-int adb_raster_blend_fwd_hits(int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
-                              const int32_t* tile_offsets, float* colors, float* alphas, int32_t* last_ids,
-                              unsigned char* hit_mask, adb_stream_t stream);
-int adb_raster_blend_bwd_hits(int W, int H, int n_per_cam, const float* splats, const int32_t* vals_sorted,
-                              const int32_t* tile_offsets, const float* alphas, const int32_t* last_ids, const float* v_colors,
-                              const float* v_alphas, float* v_splats, const unsigned char* hit_mask, adb_stream_t stream);
+                         const unsigned char* hit_mask /*may be NULL*/, adb_stream_t stream);
 /* View-batched blend pair (gridDim.z = C): splats [C,N,12] and v_splats [C,N,12] indexed by vals_sorted (c*N + gaussian)
  * directly, tile_offsets [C,T+1] from adb_raster_tile_scan_multi, colors / v_colors [C,H,W,4], alphas / last_ids / v_alphas
- * [C,H,W]; hit_mask (may be NULL) indexed like vals_sorted.  Per view the same images as the single-view _hits pair; last_ids
+ * [C,H,W]; hit_mask (may be NULL) indexed like vals_sorted.  Per view the same images as the single-view pair; last_ids
  * are absolute sorted indices.  N = 0 (empty scene): the forward writes empty images (splats may be NULL), the backward
  * returns without a launch. */
 int adb_raster_blend_fwd_multi(int N, int C, int W, int H, const float* splats, const int32_t* vals_sorted,

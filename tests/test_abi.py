@@ -105,9 +105,18 @@ def test_round2_entry_points_refuse_bad_arguments_before_touching_the_device():
     assert refused(L.adb_peer_alloc(0, None), "adb_peer_alloc")
     assert refused(L.adb_peer_export(None, None), "adb_peer_export")
     assert refused(L.adb_peer_import(None, None), "adb_peer_import")
-    assert refused(L.adb_raster_blend_fwd_hits(16, 16, 0, None, None, None, None, None, None, None, None), "null hit_mask")
-    assert refused(L.adb_raster_blend_bwd_hits(16, 16, 4, None, None, None, None, None, None, None, None, None, None),
-                   "null hit_mask")
+    hm = ctypes.c_void_p(256)                                                                  # never dereferenced
+    for mask in (None, hm):
+        assert refused(L.adb_raster_blend_fwd(0, 16, 4, None, None, None, None, None, None, mask, None),
+                       "adb_raster_blend_fwd: bad sizes")
+        assert refused(L.adb_raster_blend_fwd(16, 16, 4, None, None, None, None, None, None, mask, None),
+                       "adb_raster_blend_fwd: null pointer")
+        assert refused(L.adb_raster_blend_bwd(16, 16, -1, None, None, None, None, None, None, None, None, mask, None),
+                       "adb_raster_blend_bwd: bad sizes")
+        assert refused(L.adb_raster_blend_bwd(16, 16, 4, None, None, None, None, None, None, None, None, mask, None),
+                       "adb_raster_blend_bwd: null pointer")
+        assert refused(L.adb_raster_blend_bwd(16, 16, 4, None, None, hm, hm, hm, hm, hm, None, mask, None),
+                       "adb_raster_blend_bwd: null v_splats")
     assert refused(L.adb_raster_sh_expand_multi(4, 0, None, 3, None, None, None, None), "adb_raster_sh_expand_multi")
     assert refused(L.adb_raster_sh_expand_multi(4, 1, None, 4, None, None, None, None), "adb_raster_sh_expand_multi")  # degree > 3
     assert refused(L.adb_raster_sh_dir_bwd_multi(4, 1, None, None, 3, None, None, None, None, None, None),

@@ -274,8 +274,8 @@ def test_multi_view_exchange_algebra_matches_single_process(cuda):
 @pytest.mark.parametrize("N,W,H,view,kw", [(3000, 320, 192, 1.0, {}), (50000, 960, 544, 5.0, dict(scale_range=(0.01, 0.15))),
                                            (100000, 1920, 1080, 3.5, {})])
 def test_backward_from_the_forward_hit_mask_equals_backward_with_its_own_culling(cuda, N, W, H, view, kw):
-    """adb_raster_blend_fwd_hits / adb_raster_blend_bwd_hits: the forward records which warps each (tile, splat) entry can reach
-    and the backward builds its hit lists from that record.  Same images bit for bit; same gradients up to the order of the
+    """adb_raster_blend_fwd / adb_raster_blend_bwd with a hit_mask: the forward records which warps each (tile, splat) entry can
+    reach and the backward builds its hit lists from that record.  Same images bit for bit; same gradients up to the order of the
     floating-point REDs between tiles."""
     from artdeco_b200 import raster as R
     sc, V, K = _scene(N, W, H, seed=21, view=view, **kw)

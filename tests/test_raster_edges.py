@@ -1,7 +1,6 @@
 """The tile sort and the blend where uniform random scenes never go: tiles of up to 20000 entries (every bitonic level of the
 shared-memory sort and the in-place global-memory network), depth ties, tiles that saturate inside a long list, splats larger
-than the frame (16-bit cull radii saturated at 65535), ragged frames, and the opt-in blend variants (ADB_BLEND_TMA=1,
-ADB_BWD_SLOTS=32, ADB_BWD_OCC=3) in a child process.
+than the frame (16-bit cull radii saturated at 65535) and ragged frames.
 
 References: the C oracle (an independent radix sort; a blend that evaluates every entry with expf, without culling).
 Integer outputs are bit-exact.  Floating-point outputs are within 1e-4 of the tensor's scale (tests/helpers.py).
@@ -13,10 +12,6 @@ where last_ids or the image differs is walked again in fp64 from the oracle's in
 
 Each group also builds its nearest plausible bug from oracle outputs and asserts that it would fail the comparison."""
 import functools
-import os
-import subprocess
-import sys
-import tempfile
 
 import numpy as np
 import pytest
@@ -523,12 +518,12 @@ def test_blend_ladder_forward_backward_match_oracle(cuda, regime):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("regime", list(REGIMES))
-def test_blend_ladder_hit_mask_path(cuda, regime):
+@pytest.mark.parametrize("key", list(REGIMES) + ["frame"])
+def test_blend_ladder_hit_mask_path(cuda, key):
     """blend_forward(hits=) renders the same bits; blend_backward(hits=) matches the kernel's own culling within 2e-6; the
     last contributor of every covered pixel is marked for its warp."""
     from artdeco_b200 import raster as R
-    sc, V, K, W, H, _, _ = ladder(regime)
+    sc, V, K, W, H = _scene(key)
     st = stages(sc, V, K, W, H, cuda)
     N = len(sc["means"])
     hits = torch.full((max(1, st["n"]),), 0xAB, dtype=torch.uint8, device=cuda)
@@ -611,55 +606,12 @@ def test_blend_entry_points_refuse_misaligned_records_and_outputs():
         msg = L.adb_last_error()
         return rc == 1 and msg is not None and "16-byte aligned" in msg.decode()
 
-    fwd = lambda sp, col: L.adb_raster_blend_fwd(16, 16, 8, sp, ok, ok, col, ok, ok, None)
-    assert refused(fwd(odd, ok)) and refused(fwd(ok, odd))
-    assert refused(L.adb_raster_blend_fwd_hits(16, 16, 8, ok, ok, ok, odd, ok, ok, ok, None))
+    fwd = lambda sp, col, hm: L.adb_raster_blend_fwd(16, 16, 8, sp, ok, ok, col, ok, ok, hm, None)
+    bwd = lambda sp, vc, vs, hm: L.adb_raster_blend_bwd(16, 16, 8, sp, ok, ok, ok, ok, vc, ok, vs, hm, None)
+    for hm in (None, ok):
+        assert refused(fwd(odd, ok, hm)) and refused(fwd(ok, odd, hm))
+        assert refused(bwd(odd, ok, ok, hm)) and refused(bwd(ok, odd, ok, hm)) and refused(bwd(ok, ok, odd, hm))
     assert refused(L.adb_raster_blend_fwd_multi(8, 2, 16, 16, odd, ok, ok, ok, ok, ok, None, None))
     assert refused(L.adb_raster_blend_fwd_multi(8, 2, 16, 16, ok, ok, ok, odd, ok, ok, None, None))
-    bwd = lambda sp, vc, vs: L.adb_raster_blend_bwd(16, 16, 8, sp, ok, ok, ok, ok, vc, ok, vs, None)
-    assert refused(bwd(odd, ok, ok)) and refused(bwd(ok, odd, ok)) and refused(bwd(ok, ok, odd))
-    assert refused(L.adb_raster_blend_bwd_hits(16, 16, 8, ok, ok, ok, ok, ok, ok, ok, odd, ok, None))
     assert refused(L.adb_raster_blend_bwd_multi(8, 2, 16, 16, ok, ok, ok, ok, ok, ok, ok, odd, None, None))
 
-
-# ---- opt-in blend variants, each in its own process (the switches are read once per process) -------------------------------
-VARIANTS = {"tma": {"ADB_BLEND_TMA": "1"}, "slots32": {"ADB_BWD_SLOTS": "32"}, "occ3": {"ADB_BWD_OCC": "3"}}
-# backward bound relative to the tensor's scale: TMA staging and the occupancy bound change only the order of the REDs;
-# 32 slots also reassociate each warp's 32-pixel moment sums (one pass instead of two 16-pixel halves and a shuffle), and
-# the conversion to splat-centred moments (ex (ex S0 - 2 Sx) + Sxx, ex up to 8 px) amplifies that rounding
-BWD_BOUND = {"tma": 2e-6, "slots32": 2e-5, "occ3": 2e-6}
-SWITCHES = ("ADB_BLEND_TMA", "ADB_BWD_SLOTS", "ADB_BWD_OCC", "ADB_BLEND_HITS")
-
-
-@functools.lru_cache(maxsize=None)
-def _default_render():
-    import raster_variant_child as child
-    return child.render_all(torch.device("cuda:0"))
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("variant", list(VARIANTS))
-def test_opt_in_blend_variant_matches_the_default(cuda, variant):
-    """Forward bit-identical (colours, alphas, last_ids, hit masks: prescale_record and stage_record do the same
-    arithmetic); backward within BWD_BOUND relative (the REDs arrive in another order)."""
-    if any(os.environ.get(s) for s in SWITCHES):
-        pytest.skip("a blend switch is set in this process: the in-process reference would not be the default path")
-    ref = _default_render()
-    env = {k: v for k, v in os.environ.items() if k not in SWITCHES}
-    env.update(VARIANTS[variant])
-    script = os.path.join(os.path.dirname(os.path.abspath(__file__)), "raster_variant_child.py")
-    with tempfile.TemporaryDirectory() as d:
-        out = os.path.join(d, "out.pt")
-        p = subprocess.run([sys.executable, script, out], env=env, capture_output=True, text=True, timeout=300)
-        assert p.returncode == 0, p.stdout[-2000:] + p.stderr[-4000:]
-        got = torch.load(out)
-    assert sorted(got) == sorted(ref)
-    worst = 0.0
-    for k in ref:
-        if k.startswith("bwd"):
-            e = rel_err(got[k], ref[k])
-            worst = max(worst, e)
-            assert e < BWD_BOUND[variant], (variant, k, e)
-        else:
-            assert torch.equal(got[k], ref[k]), (variant, k)
-    print(f"[{variant}] {len(ref)} outputs; forward bit-identical, backward max rel err {worst:.2e}")

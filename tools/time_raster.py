@@ -1,5 +1,5 @@
 """Per-stage live timing (CUDA events on the launching stream) of the rasterizer step at the bench workload, without the
-e2e / MASt3R / CPU legs.  ADB_BWD_SLOTS=16|32 selects the A/B variant."""
+e2e / MASt3R / CPU legs."""
 import json
 import os
 import sys
@@ -31,7 +31,7 @@ def step():
     radii, splats, tpg = R.project(t["means"], t["quats"], t["scales"], t["opacities"], t["sh"], 3, Vd, Kd, campos, W, H,
                                    0.01, 0.01, 1e10, 0.0, tile_counts=cnt)
     keys, vals, offs, n = R.intersect(radii, splats, tpg, W, H, counts=cnt)
-    hits = R.new_hit_mask(vals)                     # ADB_BLEND_HITS=0: both kernels cull on their own
+    hits = R.new_hit_mask(vals)
     colors, alphas, last = R.blend_forward(W, H, N, splats, vals, offs, hits=hits)
     v_splats = R.blend_backward(W, H, N, splats, vals, offs, alphas, last, vcd, vad, hits=hits)
     _lib.call("adb_raster_project_bwd", N, _lib.ptr(t["means"]), _lib.ptr(t["quats"]), _lib.ptr(t["scales"]),
@@ -57,6 +57,5 @@ for _ in range(steps):
 torch.cuda.synchronize()
 tot = _lib.TIMER.totals_ms()
 _lib.TIMER = None
-print(json.dumps({"bwd_slots": os.environ.get("ADB_BWD_SLOTS", "16"),
-                  "N": N, "W": W, "H": H, "ms_per_step": ms, "n_isect": info["n_isect"],
+print(json.dumps({"N": N, "W": W, "H": H, "ms_per_step": ms, "n_isect": info["n_isect"],
                   "stage_ms": {k.replace("adb_raster_", ""): round(v[0] / v[1], 4) for k, v in tot.items()}}))
