@@ -11,10 +11,11 @@
 //    on small splats: 51 % of the lanes of an evaluated (warp, splat) pair contribute at the BASELINE workload);
 //  * the tile's slice of the depth-sorted list is staged 256 splats at a time as 48 B shared-memory records, the conic
 //    pre-scaled by log2(e)/2 so that sigma is 5 FP32 ops and alpha is one MUFU.EX2 without a range-reduction multiply;
-//  * WARP-COOPERATIVE CULLING: lane l tests splat l of a 32-chunk against the warp's block (integer radius box, then the
-//    exact minimum of sigma over the block's rectangle against ln(255 o)); a ballot compacts the survivors into the
-//    warp's private 16-bit hit list, padded to a multiple of four with a never-visible dummy record so the evaluation
-//    loop is unrolled by four with one LDS.64 of list entries and no remainder code;
+//  * CULLING AT STAGING: the thread that stages a record also computes its 8-bit warp mask (which of the tile's eight 8x4
+//    blocks the ellipse sigma <= ln(255 o) can reach, intersected with the integer-radius box; see warp_mask).  Each warp
+//    then compacts the slots carrying its bit into a private 16-bit hit list with one ballot per 32 slots, padded to a
+//    multiple of four with a never-visible dummy record so the evaluation loop is unrolled by four with one LDS.64 of list
+//    entries and no remainder code;
 //  * the evaluation bodies are branch-free (predicated selects), so the four unrolled bodies interleave;
 //  * BACKWARD — the per-splat reduction over the warp's 32 pixels is NOT a shuffle butterfly.  All ten per-Gaussian
 //    sums are dot products of two per-(pixel,splat) scalars with weights that do not depend on the splat:
@@ -50,10 +51,67 @@ __device__ __forceinline__ float rcp_approx(float x) {
     return y;
 }
 
-// warp block geometry: warp w covers pixels x in [bx*16 + (w&1)*8, +8), y in [by*16 + (w>>1)*4, +4)
-struct WarpRect {
-    float xlo, xhi, ylo, yhi;  // pixel-centre range
-};
+__device__ __forceinline__ float sqrt_approx(float x) {
+    float y;
+    asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+    return y;
+}
+
+// Warp mask of a staged record (A, B as in stage_record) over the tile whose first pixel centre is (tx0, ty0): bit w is set
+// when the splat can pass the per-pixel test 0 <= sigma2 <= smax2 somewhere in warp w's 8x4 block, i.e. pixel centres
+// x in tx0 + 8 (w & 1) + [0, 7], y in ty0 + 4 (w >> 1) + [0, 3].  Two conservative tests, ANDed:
+//  1. the integer-radius box written by the projection (outside it alpha < 1/255 by construction of the radius);
+//  2. per 4-pixel row band, the x-interval of the ellipse {sigma2 <= S} over the band's continuous y-range against the two
+//     column halves.  For a row offset e = y - my the ellipse's x-range is mx + (-b2 e -+ sqrt(4 ha S - D e^2)) / (2 ha),
+//     D = 4 ha hc - b2^2; the right end is concave in e, so its maximum over the band is at its stationary point (the
+//     ellipse's rightmost point, e = -b2 xm / (2 hc) with xm the x half-extent) clamped to the band, the left end likewise.
+// S is smax2 widened by the rounding error of the per-pixel fp32 sigma2 (terms up to kappa = 4 ha hc / D times sigma2 cancel
+// in it) plus relative and absolute slack, and the band and the interval are widened by the rounding of the coordinates, so
+// the mask keeps every block that holds a pixel passing the per-pixel test: the image is the same as with no culling.
+// A conic that is not positive definite, or too ill-conditioned to bound its rounding, falls back to the box.
+// About 110 thread-instructions per record, computed once by the staging thread instead of by every warp.
+__device__ __forceinline__ unsigned warp_mask(const float4& A, const float4& B, float tx0, float ty0) {
+    const unsigned pr = __float_as_uint(B.w);
+    // 65535 is the saturation value written by the projection: treat it as unbounded
+    const float rx = (pr & 0xffffu) == 0xffffu ? 3.0e38f : (float)(pr & 0xffffu);
+    const float ry = (pr >> 16) == 0xffffu ? 3.0e38f : (float)(pr >> 16);
+    const float mx = A.x, my = A.y, ha = A.z, b = A.w, hc = B.x;
+    const float D = 4.f * ha * hc - b * b;
+    const float kap = __fdividef(4.f * ha * hc, D);
+    const bool conic_ok = ha > 0.f && hc > 0.f && D > 0.f && kap < 1.0e6f;
+    const float S = fmaxf(0.f, B.z * (1.0002f + 2.0e-6f * kap) + 2.0e-4f);
+    const float pad = 1.0e-3f + 2.0e-6f * fmaxf(fabsf(mx), fabsf(my));
+    const float rD = rcp_approx(D);
+    const float S4a = 4.f * ha * S;
+    const float xm = sqrt_approx(4.f * hc * S * rD), ym = sqrt_approx(S4a * rD);
+    const float eR = -0.5f * b * xm * rcp_approx(hc);              // row offset of the rightmost point; leftmost at -eR
+    const float r2a = rcp_approx(2.f * ha);
+    unsigned mask = 0u;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const float xlo = tx0 + 8.f * h, xhi = xlo + 7.f;
+        const unsigned cols = (mx + rx >= xlo && mx - rx <= xhi) ? (0x55u << h) : 0u;
+        mask |= cols;
+    }
+    unsigned rows = 0u;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const float ylo = ty0 + 4.f * k, yhi = ylo + 3.f;
+        if (!(my + ry >= ylo && my - ry <= yhi)) continue;
+        if (!conic_ok) { rows |= 3u << (2 * k); continue; }
+        const float e0 = ylo - my - pad, e1 = yhi - my + pad;
+        if (e0 > ym || e1 < -ym) continue;
+        const float cR = fminf(e1, fmaxf(e0, eR)), cL = fminf(e1, fmaxf(e0, -eR));
+        const float xR = mx + (sqrt_approx(fmaxf(0.f, S4a - D * cR * cR)) - b * cR) * r2a + pad;
+        const float xL = mx - (sqrt_approx(fmaxf(0.f, S4a - D * cL * cL)) + b * cL) * r2a - pad;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const float xlo = tx0 + 8.f * h, xhi = xlo + 7.f;
+            if (xL <= xhi && xR >= xlo) rows |= 1u << (2 * k + h);
+        }
+    }
+    return mask & rows;
+}
 
 // Shared-memory record (3 x float4, 48 B stride: conflict-free for both the staging stores and the broadcast loads):
 //   A = (mx, my, ha, b2)   B = (hc, opacity, smax2, bits rx|ry<<16)   C = (r, g, b, depth | 1/depth for LEGACY)
@@ -61,8 +119,10 @@ struct WarpRect {
 //   sigma2 = log2e * sigma = dx (ha dx + b2 dy) + hc dy^2,   alpha = o * 2^(-sigma2),
 //   and  alpha >= 1/255  <=>  sigma2 <= smax2  — one compare replaces the alpha test (the two differ only where
 //   o 2^(-sigma2) is within an ulp of 1/255, the same measure-zero band in which ex2.approx and the oracle's expf disagree).
+// When `mask` is not NULL it receives the record's warp mask over the tile whose first pixel centre is (tx0, ty0).
 template <bool LEGACY>
-__device__ __forceinline__ void stage_record(float4* __restrict__ rec, const float* __restrict__ splats, int g) {
+__device__ __forceinline__ void stage_record(float4* __restrict__ rec, const float* __restrict__ splats, int g,
+                                             unsigned char* __restrict__ mask, float tx0, float ty0) {
     const float4* p = reinterpret_cast<const float4*>(splats + (size_t)g * ADB_SPLAT_STRIDE);
     float4 A = __ldg(p), B = __ldg(p + 1), C = __ldg(p + 2);
     A.z *= 0.5f * LOG2E;
@@ -73,6 +133,7 @@ __device__ __forceinline__ void stage_record(float4* __restrict__ rec, const flo
     rec[0] = A;
     rec[1] = B;
     rec[2] = C;
+    if (mask) *mask = (unsigned char)warp_mask(A, B, tx0, ty0);
 }
 
 __device__ __forceinline__ void write_dummy(float4* __restrict__ rec) {
@@ -81,83 +142,9 @@ __device__ __forceinline__ void write_dummy(float4* __restrict__ rec) {
     rec[2] = make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
-// Can the splat reach alpha >= 1/255 anywhere in the warp's block?  Two conservative tests:
-//  1. the integer-radius box written by the projection (outside it alpha < 1/255 by construction of the radius);
-//  2. the exact minimum of sigma2(d) = ha dx^2 + hc dy^2 + b2 dx dy over the block's pixel-centre rectangle against smax2 —
-//     the same bound the per-pixel pre-test uses, so a culled splat would have failed that pre-test on every pixel of the
-//     block and the image is unchanged.  ~1.5 warp-instructions per (warp, splat) because 32 splats are tested per
-//     instruction, against ~35 (forward) / ~55 (backward) for the evaluation it avoids.
-__device__ __forceinline__ bool splat_box_hits(const float4& A, const float4& B, const WarpRect& r) {
-    const unsigned pr = __float_as_uint(B.w);
-    // 65535 is the saturation value written by the projection: treat it as unbounded
-    const float rx = (pr & 0xffffu) == 0xffffu ? 3.0e38f : (float)(pr & 0xffffu);
-    const float ry = (pr >> 16) == 0xffffu ? 3.0e38f : (float)(pr >> 16);
-    return (A.x + rx >= r.xlo) && (A.x - rx <= r.xhi) && (A.y + ry >= r.ylo) && (A.y - ry <= r.yhi);
-}
-__device__ __forceinline__ bool splat_exact_hits(const float4& A, const float4& B, const WarpRect& r) {
-    const float x0 = r.xlo - A.x, x1 = r.xhi - A.x, y0 = r.ylo - A.y, y1 = r.yhi - A.y;
-    if (x0 <= 0.f && x1 >= 0.f && y0 <= 0.f && y1 >= 0.f) return true;   // centre inside the block
-    const float ha = A.z, b = A.w, hc = B.x;
-    const float nb_c = -0.5f * __fdividef(b, hc), nb_a = -0.5f * __fdividef(b, ha);
-    // minimum over each edge (1-D quadratic, minimiser clamped to the edge); the rectangle's minimum is on its boundary
-    float m;
-    {
-        const float dy0 = fminf(y1, fmaxf(y0, nb_c * x0)), dy1 = fminf(y1, fmaxf(y0, nb_c * x1));
-        const float q0 = ha * x0 * x0 + hc * dy0 * dy0 + b * x0 * dy0;
-        const float q1 = ha * x1 * x1 + hc * dy1 * dy1 + b * x1 * dy1;
-        m = fminf(q0, q1);
-    }
-    {
-        const float dx0 = fminf(x1, fmaxf(x0, nb_a * y0)), dx1 = fminf(x1, fmaxf(x0, nb_a * y1));
-        const float q0 = ha * dx0 * dx0 + hc * y0 * y0 + b * dx0 * y0;
-        const float q1 = ha * dx1 * dx1 + hc * y1 * y1 + b * dx1 * y1;
-        m = fminf(m, fminf(q0, q1));
-    }
-    // rounding slack: the per-pixel test is sigma2 <= smax2 in the same fp32 arithmetic
-    return m <= B.z * 1.0001f + 1e-4f;
-}
-
-// Builds the warp's hit list for the staged batch (ascending slot order), padded to a multiple of 4 with DUMMY.
-// `limit`: only slots s with s >= limit are considered (the backward skips splats behind the warp's last contributor).
-// Two dense phases: (1) the cheap integer-radius box test on all slots, survivors compacted into the list; (2) the exact
-// ellipse-vs-rectangle test on the survivors only (46 % of the slots at the bench workload), 32 per instruction, compacted in
-// place (the write index never passes the read index).  A single fused test would run the expensive half with most lanes idle.
-__device__ __forceinline__ int build_hit_list(const float4* __restrict__ sRec, unsigned short* __restrict__ list,
-                                              int bsize, int limit, const WarpRect& rect, int lane) {
-    const unsigned lt_mask = (1u << lane) - 1u;
-    int nbox = 0;
-    for (int c0 = (limit > 0 ? (limit & ~31) : 0); c0 < bsize; c0 += 32) {
-        const int s = c0 + lane;
-        bool hit = false;
-        if (s < bsize && s >= limit) hit = splat_box_hits(sRec[s * 3], sRec[s * 3 + 1], rect);
-        const unsigned mask = __ballot_sync(FULL, hit);
-        if (hit) list[nbox + __popc(mask & lt_mask)] = (unsigned short)s;
-        nbox += __popc(mask);
-    }
-    __syncwarp();
-    int nhit = 0;
-    for (int c0 = 0; c0 < nbox; c0 += 32) {
-        const int k = c0 + lane;
-        int s = 0;
-        bool hit = false;
-        if (k < nbox) {
-            s = list[k];
-            hit = splat_exact_hits(sRec[s * 3], sRec[s * 3 + 1], rect);
-        }
-        const unsigned mask = __ballot_sync(FULL, hit);     // every lane has read its entry before any lane overwrites one
-        if (hit) list[nhit + __popc(mask & lt_mask)] = (unsigned short)s;
-        nhit += __popc(mask);
-        __syncwarp();
-    }
-    if (lane < 3) list[nhit + lane] = (unsigned short)DUMMY;
-    __syncwarp();
-    return nhit;
-}
-
-// The backward's hit list from the forward's per-entry warp masks (bit w of hit_mask[sorted index] = warp w's block is hit):
-// the forward has already run both tests on every entry a warp can need again — the backward only revisits entries up to the
-// warp's last contributor, all of which lie in batches that warp went through — so the backward replaces ~150 instructions
-// per 32 slots by a table look-up and a compaction.  sM[slot] = mask of the staged batch (slot order = back to front).
+// A warp's hit list from the staged batch's warp masks (sM[slot], bit w = warp w's block is hit), ascending slot order,
+// padded to a multiple of 4 with DUMMY.  `limit`: only slots s >= limit are considered (the backward skips splats behind
+// the warp's last contributor).
 __device__ __forceinline__ int build_hit_list_from_mask(const unsigned char* __restrict__ sM, unsigned short* __restrict__ list,
                                                         int bsize, int limit, int warp, int lane) {
     const unsigned lt_mask = (1u << lane) - 1u;
@@ -193,7 +180,7 @@ blend_fwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
     constexpr float MAXA = LEGACY ? ADB_MAX_ALPHA_INRIA : ADB_MAX_ALPHA;
     __shared__ __align__(16) float4 sRec[(BLOCK + 1) * 3];
     __shared__ __align__(8) unsigned short sList[NWARP][LIST_STRIDE];
-    __shared__ unsigned sMask[BLOCK / 4];       // byte s = warp mask of slot s of the current batch (hit_mask != NULL)
+    __shared__ unsigned char sM[BLOCK];         // warp masks of the staged batch
 
     const int tw = (W + ADB_TILE - 1) / ADB_TILE;
     const int tile = blockIdx.y * tw + blockIdx.x;
@@ -202,24 +189,10 @@ blend_fwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
     const int j = x0 + (lane & 7), i = y0 + (lane >> 3);
     const bool inside = (i < H && j < W);
     const float px = (float)j + 0.5f, py = (float)i + 0.5f;
-    const WarpRect rect{(float)x0 + 0.5f, (float)x0 + 7.5f, (float)y0 + 0.5f, (float)y0 + 3.5f};
+    const float tx0 = (float)(blockIdx.x * ADB_TILE) + 0.5f, ty0 = (float)(blockIdx.y * ADB_TILE) + 0.5f;
     const size_t view_pix = (size_t)blockIdx.z * H * W;
     const int orow = blockIdx.z * (gridDim.x * gridDim.y + 1) + tile;
     const int start = tile_offsets[orow], end = tile_offsets[orow + 1];
-    if (tid < BLOCK / 4) sMask[tid] = 0u;
-    // Writes the finished batch's warp masks to hit_mask[start + pb*BLOCK ...] and clears the table (one thread per word, so the
-    // clear cannot race with the read; the barrier that follows orders it before the next batch's atomics).
-    auto flush_mask = [&](int pb) {
-        if (tid < BLOCK / 4) {
-            const unsigned w = sMask[tid];
-            sMask[tid] = 0u;
-            const int i0 = start + pb * BLOCK + tid * 4;
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-                if (i0 + k < end) hit_mask[i0 + k] = (unsigned char)((w >> (8 * k)) & 0xffu);
-        }
-    };
-    int pending = -1;                            // batch whose masks are complete but not written yet (block-uniform)
     if (tid == 0) write_dummy(sRec + DUMMY * 3);
     const int nb = (end - start + BLOCK - 1) / BLOCK;
 
@@ -231,23 +204,18 @@ blend_fwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
     bool done = !inside;
     for (int b = 0; b < nb; ++b) {
         const int n_done = __syncthreads_count(done);    // also: every warp has finished reading the previous batch
-        if (hit_mask && pending >= 0) { flush_mask(pending); pending = -1; }
         const int bstart = start + b * BLOCK;
         const int idx = bstart + tid;
         if (n_done >= BLOCK) break;
-        if (idx < end) stage_record<LEGACY>(sRec + tid * 3, splats, record_index(vals[idx], wrap));
+        if (idx < end) {
+            stage_record<LEGACY>(sRec + tid * 3, splats, record_index(vals[idx], wrap), sM + tid, tx0, ty0);
+            if (hit_mask) hit_mask[idx] = sM[tid];
+        }
         __syncthreads();
-        pending = b;
         const int bsize = min(BLOCK, end - bstart);
         if (__all_sync(FULL, done)) continue;
         unsigned short* list = sList[warp];
-        const int nhit = build_hit_list(sRec, list, bsize, 0, rect, lane);
-        if (hit_mask) {
-            for (int k = lane; k < nhit; k += 32) {
-                const unsigned sl = list[k];
-                atomicOr(&sMask[sl >> 2], 1u << (((sl & 3u) << 3) + warp));
-            }
-        }
+        const int nhit = build_hit_list_from_mask(sM, list, bsize, 0, warp, lane);
         int cur_t = -1;
         const int nq = (nhit + 3) >> 2;
         for (int q = 0; q < nq; ++q) {
@@ -277,10 +245,6 @@ blend_fwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
             if ((q & 1) && __all_sync(FULL, done)) break;
         }
         if (cur_t >= 0) cur = bstart + cur_t;
-    }
-    if (hit_mask && pending >= 0) {              // the loop ran to its end: the last batch's masks are still in shared memory
-        __syncthreads();
-        flush_mask(pending);
     }
     if (inside) {
         const size_t pix = view_pix + (size_t)i * W + j;
@@ -339,7 +303,7 @@ blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
     const int j = x0 + (lane & 7), i = y0 + (lane >> 3);
     const bool inside = (i < H && j < W);
     const float px = (float)j + 0.5f, py = (float)i + 0.5f;
-    const WarpRect rect{(float)x0 + 0.5f, (float)x0 + 7.5f, (float)y0 + 0.5f, (float)y0 + 3.5f};
+    const float tx0 = (float)(blockIdx.x * ADB_TILE) + 0.5f, ty0 = (float)(blockIdx.y * ADB_TILE) + 0.5f;
     // view row of tile_offsets by a 32-bit index (a 64-bit pointer bump here costs the 64-register build one more spill slot)
     const int orow = blockIdx.z * (gridDim.x * gridDim.y + 1) + tile;
     const int start = tile_offsets[orow], end = tile_offsets[orow + 1];
@@ -378,15 +342,14 @@ blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
         if (idx >= start) {
             const int g = record_index(vals[idx], wrap);
             sG[tid] = g;
-            stage_record<LEGACY>(sRec + tid * 3, splats, g);
+            stage_record<LEGACY>(sRec + tid * 3, splats, g, hit_mask ? nullptr : sM + tid, tx0, ty0);
+            if (hit_mask) sM[tid] = hit_mask[idx];
         }
-        if (hit_mask && idx >= start) sM[tid] = hit_mask[idx];
         __syncthreads();
         // a splat at slot s contributes to this warp only if batch_end - s <= warp_bin_final
         const int limit = max(0, batch_end - warp_bin_final);
         if (limit >= bsize) continue;
-        const int nhit = hit_mask ? build_hit_list_from_mask(sM, list, bsize, limit, warp, lane)
-                                  : build_hit_list(sRec, list, bsize, limit, rect, lane);
+        const int nhit = build_hit_list_from_mask(sM, list, bsize, limit, warp, lane);
         const int tmin = inside ? batch_end - bin_final : (1 << 30);   // lane-valid iff t >= tmin
         for (int g0 = 0; g0 < nhit; g0 += SLOTS) {
             const int ng = min(SLOTS, nhit - g0);
@@ -452,7 +415,7 @@ blend_bwd_kernel(int W, int H, const float* __restrict__ splats, const int32_t* 
                 const float4 A = sRec[t * 3];
                 float* dst = v_splats + (size_t)sG[t] * ADB_SPLAT_STRIDE;
                 // dx = ex - lx, dy = ey - ly with (lx, ly) the integer pixel offset inside the block
-                const float ex = A.x - rect.xlo, ey = A.y - rect.ylo;
+                const float ex = A.x - ((float)x0 + 0.5f), ey = A.y - ((float)y0 + 0.5f);
                 if (r_half == 0) {
                     if (S0 != 0.f || Sx != 0.f || Sy != 0.f || Sxx != 0.f || Sxy != 0.f) {
                         const float Mx = fmaf(ex, S0, -Sx), My = fmaf(ey, S0, -Sy);
