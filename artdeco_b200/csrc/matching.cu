@@ -61,8 +61,12 @@ match_prep_kernel(int H, int W, const float* __restrict__ X11, const float* __re
     const size_t q = (size_t)b * H * W + n;
     unit3(X21 + q * 3, pts + q * 3);
     const long long li = idx_init ? idx_init[q] : (long long)n;
-    p_init[q * 2] = (float)(li % W);
-    p_init[q * 2 + 1] = (float)(li / W);
+    // lin_to_pixel (utils_matching.py:99-103) is torch's % and //, which floor: a negative index maps to
+    // (li mod W in [0, W), floor(li / W)), not C's truncated quotient and signed remainder
+    long long vi = li / W, ui = li - vi * W;
+    if (ui < 0) { ui += W; --vi; }
+    p_init[q * 2] = (float)ui;
+    p_init[q * 2 + 1] = (float)vi;
 }
 
 struct Bilin {
@@ -189,8 +193,9 @@ refine_matches_kernel(int H, int W, int n_pts, const __half* __restrict__ D11, c
     const size_t pstep = PLANAR ? 1 : (F / 8);           // distance between neighbouring pixels' first chunks
     long long u0 = p1[q * 2], v0 = p1[q * 2 + 1];
     long long u_new = u0, v_new = v0;
-    // numeric_limits<Half>::min() (smallest positive normal, matching_kernels.cu:50): scores at or below it never win
-    float max_score = 6.103515625e-05f;
+    // matching_kernels.cu:47 starts from ::cuda::std::numeric_limits<c10::Half>::min(); libcu++ does not specialise
+    // numeric_limits for c10::Half, so that is Half() == 0: any positive score wins, a score <= 0 never does
+    float max_score = 0.f;
     for (int d = dilation_max; d > 0; --d) {
         const int rd = radius * d;
         const int cnt = (2 * rd) / d + 1;     // i = 0, d, 2d, .. < 2rd+1
