@@ -21,7 +21,7 @@ There is no CPU implementation: every operator raises unless a CUDA sm_90 device
 ``libartdeco_b200.so`` are available.
 """
 from . import _lib  # noqa: F401
-from . import adam, covmlp, cull, densify, evaluate, factor_graph, gn, keyframe, knn, legacy, lpips, mapper, mast3r, matching, multiview, optimizers, parallel, peer, raster, reanchor, scene, tracking, voxel  # noqa: F401  (each registers its C signatures)
+from . import adam, covmlp, cull, densify, evaluate, factor_graph, gn, keyframe, knn, legacy, lpips, mapper, mast3r, matching, multiview, optimizers, parallel, raster, reanchor, scene, tracking, voxel  # noqa: F401  (each registers its C signatures)
 from .adam import adamUpdate, adamUpdateBasic  # noqa: F401
 from .covmlp import cov_mlp_modulate  # noqa: F401
 from .cull import lod_cull, lod_select, weed_out_mask  # noqa: F401

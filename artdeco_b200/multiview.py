@@ -11,8 +11,7 @@ Design:
     host sync (intersection buffers are sized by a capacity measured once) and is captured in ONE CUDA graph;
   * gradients are produced by the multi-view backward kernels (parameters read once, gradients written once);
   * multi-GPU: 12 B colour gradients all-gathered, 11 geometry floats all-reduced, both overlapped with the backward
-    kernels, instead of a dense [N,59] all-reduce — by ``parallel.MultiViewExchange`` (NCCL, default) or ``peer.PeerExchange``
-    (this library's kernels storing into the other GPUs' memory over NVLink; ``exchange_kind="peer"`` / ``ADB_EXCHANGE=peer``).
+    kernels, instead of a dense [N,59] all-reduce — by ``parallel.MultiViewExchange`` (NCCL).
 """
 from __future__ import annotations
 
@@ -20,7 +19,7 @@ import torch
 
 from . import _lib
 from . import raster as R
-from .peer import make_exchange
+from .parallel import MultiViewExchange
 
 KEYS = ("means", "quats", "scales", "opacities", "sh")
 
@@ -28,12 +27,10 @@ KEYS = ("means", "quats", "scales", "opacities", "sh")
 class MultiViewStep:
     def __init__(self, params: dict, viewmats: torch.Tensor, Ks: torch.Tensor, W: int, H: int, world: int = 1,
                  sh_degree: int = 3, eps2d: float = 0.01, near: float = 0.01, far: float = 1e10, radius_clip: float = 0.0,
-                 graph: bool = True, capacity_margin: float = 1.25, overlap_views: bool = False,  # no effect
-                 exchange_kind: str | None = None):
+                 graph: bool = True, capacity_margin: float = 1.25, overlap_views: bool = False):  # overlap_views: no effect
         """``params``: dict of the five parameter tensors on the device; ``viewmats [C,4,4]``, ``Ks [C,3,3]``: the LOCAL
-        views (``parallel.views_for_rank``).  ``world`` > 1 needs an initialised process group; ``exchange_kind``: "nccl"
-        (library collectives, the default) or "peer" (this library's kernels over NVLink peer memory); ``ADB_EXCHANGE`` sets
-        the default (``peer.make_exchange``)."""
+        views (``parallel.views_for_rank``).  ``world`` > 1 needs an initialised process group, whose ranks then exchange
+        gradients through ``parallel.MultiViewExchange``."""
         _lib.require_cuda(params["means"])
         self.p = {k: params[k].detach().contiguous() for k in KEYS}
         self.dev = self.p["means"].device
@@ -52,8 +49,7 @@ class MultiViewStep:
         self.v_colors = torch.zeros(C, H, W, 4, dtype=torch.float32, device=dev)     # static upstream-gradient buffers
         self.v_alphas = torch.zeros(C, H, W, dtype=torch.float32, device=dev)
         self.world = world
-        self.exchange = make_exchange(N, C, dev, kind=exchange_kind) if world > 1 else None
-        self._fused_push = getattr(self.exchange, "fused_mask", False)
+        self.exchange = MultiViewExchange(N, C, dev) if world > 1 else None
         self.grads = {"v_sh": torch.empty(N, 16, 3, dtype=torch.float32, device=dev)}
         if self.exchange is not None:
             self.grads.update(self.exchange.views)          # geometry gradients live in the all-reduce bucket
@@ -110,17 +106,12 @@ class MultiViewStep:
         if c == 0:
             self._project()
         col, alp, _ = self._raster(slice(c, c + 1), capacity)
-        if not self._fused_push:
-            R.mask_rgb_grad(self.splats[c], self.v_splats[c], self.grads["g_rgb"][c])
+        R.mask_rgb_grad(self.splats[c], self.v_splats[c], self.grads["g_rgb"][c])
         return col[0], alp[0]
 
     def _gather_view(self, c):
         """Hands local view c's colour gradient to the exchange as soon as its blend backward has been issued."""
-        campos = self.P if c == 0 else None
-        if self._fused_push:
-            self.exchange.push_view(c, self.splats[c], self.v_splats[c], campos)       # mask fused with the broadcast
-        else:
-            self.exchange.start_gather_view(c, self.grads["g_rgb"][c], campos)
+        self.exchange.start_gather_view(c, self.grads["g_rgb"][c], self.P if c == 0 else None)
 
     def _backward(self):
         p = self.p

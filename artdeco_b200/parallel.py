@@ -1,9 +1,9 @@
 """Host-side multi-GPU plumbing for the two places the hot path shards (SURVEY.md §8e): one process per GPU,
 ``torch.distributed`` (NCCL on GPUs; gloo in the CPU tests).
 
-* rasterizer, view-parallel: every rank holds a replica of the Gaussians and renders its own views; the per-Gaussian
-  gradients of all parameters live in ONE flat ``[N*59]`` bucket (the backward kernel writes straight into views of it),
-  so a step costs exactly one all-reduce;
+* rasterizer, view-parallel: every rank holds a replica of the Gaussians and renders its own views; a step gathers the
+  12-byte colour gradients of every view and sums the 11 geometry floats per Gaussian over the ranks
+  (``MultiViewExchange``);
 * MASt3R: independent pairs are split contiguously across ranks, no collective.
 """
 from __future__ import annotations
@@ -11,30 +11,7 @@ from __future__ import annotations
 import torch
 import torch.distributed as dist
 
-GRAD_FIELDS = (("means", 3), ("quats", 4), ("scales", 3), ("opacities", 1), ("sh", 48))
-GRAD_FLOATS = sum(m for _, m in GRAD_FIELDS)  # 59
-
-
-class GradBucket:
-    """Flat fp32 buffer + per-parameter views ([N,3], [N,4], [N,3], [N], [N,16,3])."""
-
-    def __init__(self, n_gaussians: int, device):
-        self.n = n_gaussians
-        self.flat = torch.zeros(n_gaussians * GRAD_FLOATS, dtype=torch.float32, device=device)
-        self.views = {}
-        o = 0
-        for name, m in GRAD_FIELDS:
-            v = self.flat[o:o + n_gaussians * m]
-            self.views[name] = v.view(n_gaussians, m) if m > 1 else v
-            o += n_gaussians * m
-        self.views["sh"] = self.views["sh"].view(n_gaussians, 16, 3)
-
-    def all_reduce(self):
-        """Sum over ranks (the multi-view step's semantics: loss = sum of the per-view losses)."""
-        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
-            dist.all_reduce(self.flat)
-        return self
-
+GRAD_FLOATS = 59    # dense per-Gaussian gradient the exchange replaces: means 3, quats 4, scales 3, opacity 1, SH 48
 
 GEOM_FIELDS = (("v_means", 3), ("v_quats", 4), ("v_scales", 3), ("v_opac", 1))
 GEOM_FLOATS = sum(m for _, m in GEOM_FIELDS)  # 11
@@ -52,8 +29,7 @@ class MultiViewExchange:
         colour's gradient through the view direction is added per rank for its local views, ``adb_raster_sh_dir_bwd_multi``).
     Both collectives are asynchronous: the gather overlaps the geometry kernels, the reduce overlaps the expansion
     (``raster.multi_view_backward``).  Result on every rank: exactly the sum over all views of the single-view gradients.
-    Works with NCCL (GPU) and gloo (CPU tests).  ``peer.PeerExchange`` is the same exchange by this library's own kernels over
-    NVLink peer memory (opt-in, see ``peer.make_exchange``)."""
+    Works with NCCL (GPU) and gloo (CPU tests)."""
 
     def __init__(self, n_gaussians: int, views_local: int, device, group=None):
         self.n = n_gaussians

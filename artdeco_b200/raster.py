@@ -444,7 +444,7 @@ def multi_view_backward(means, quats, scales, sh, sh_degree, viewmats, Ks, campo
 
     ``out``: optional dict of preallocated gradient tensors (``v_means [N,3], v_quats [N,4], v_scales [N,3], v_opac [N],
     v_sh [N,16,3]``), e.g. views of a flat communication bucket.
-    ``exchange`` (multi-GPU; ``peer.PeerExchange`` or ``parallel.MultiViewExchange``): the colour gradients of the local views
+    ``exchange`` (multi-GPU; a ``parallel.MultiViewExchange``): the colour gradients of the local views
     are gathered while the geometry kernels run, the 11 geometry floats are summed over ranks while the SH gradient of EVERY
     rank's views is expanded; ``None`` = single process.  Returns (v_means, v_quats, v_scales, v_opac, v_sh, v_viewmats[C,4,4],
     v_campos[C,3] of the local views)."""
@@ -471,18 +471,10 @@ def multi_view_backward(means, quats, scales, sh, sh_degree, viewmats, Ks, campo
         if exchange is not None:
             mask_rgb_grad(splats, v_splats, g_rgb)
             exchange.start_gather(g_rgb, Pc)
-    # an exchange with separate input / result buffers (peer.PeerExchange): the kernel writes this rank's partial sums into
-    # `views_in`, the reduced gradients appear in `views`
-    gin = getattr(exchange, "views_in", None) if exchange is not None else None
-    pm, pq, ps, po = (gin["v_means"], gin["v_quats"], gin["v_scales"], gin["v_opac"]) if gin is not None else \
-        (v_means, v_quats, v_scales, v_opac)
     _lib.call("adb_raster_project_bwd_multi", N, Cn, _lib.ptr(means), _lib.ptr(quats), _lib.ptr(scales), _lib.ptr(Vc),
-              _lib.ptr(Kc), W, H, _lib.ptr(radii), _lib.ptr(splats), _lib.ptr(v_splats), _lib.ptr(pm),
-              _lib.ptr(pq), _lib.ptr(ps), _lib.ptr(po), _lib.ptr(g_rgb) if exchange is None else None, _lib.ptr(v_views),
-              _lib.stream())
-    if gin is not None:
-        gout = exchange.views
-        v_means, v_quats, v_scales, v_opac = gout["v_means"], gout["v_quats"], gout["v_scales"], gout["v_opac"]
+              _lib.ptr(Kc), W, H, _lib.ptr(radii), _lib.ptr(splats), _lib.ptr(v_splats), _lib.ptr(v_means),
+              _lib.ptr(v_quats), _lib.ptr(v_scales), _lib.ptr(v_opac), _lib.ptr(g_rgb) if exchange is None else None,
+              _lib.ptr(v_views), _lib.stream())
     if exchange is None:
         _lib.call("adb_raster_sh_bwd_multi", N, Cn, _lib.ptr(means), _lib.ptr(sh), int(sh_degree), _lib.ptr(Pc),
                   _lib.ptr(g_rgb), _lib.ptr(v_sh), _lib.ptr(v_means), 1, 0, 0, _lib.ptr(v_campos), _lib.stream())
@@ -492,7 +484,7 @@ def multi_view_backward(means, quats, scales, sh, sh_degree, viewmats, Ks, campo
     # carries it; only the outer product basis(dir) (x) v_rgb needs every rank's colour gradients, and that expansion — the
     # part every rank repeats for all views — then runs without the SH coefficients and the basis gradients.
     _lib.call("adb_raster_sh_dir_bwd_multi", N, Cn, _lib.ptr(means), _lib.ptr(sh), int(sh_degree), _lib.ptr(Pc), _lib.ptr(splats),
-              _lib.ptr(v_splats), _lib.ptr(pm), _lib.ptr(v_campos), _lib.stream())
+              _lib.ptr(v_splats), _lib.ptr(v_means), _lib.ptr(v_campos), _lib.stream())
     exchange.start_reduce()                       # geometry sums (v_means | v_quats | v_scales | v_opac), overlaps the expansion
     g_all, P_all = exchange.wait_gather()
     _lib.call("adb_raster_sh_expand_multi", N, int(g_all.shape[0]), _lib.ptr(means), int(sh_degree), _lib.ptr(P_all),

@@ -618,37 +618,6 @@ int adb_upsample2x_nhwc(int B, int Hin, int Win, int C, int Hout, int Wout, cons
 int adb_head_postprocess(int B, int H, int W, const float* pts, const float* lf, long long ld_lf, int n_desc, float* pts3d,
                          float* conf, float* desc, float* desc_conf, adb_stream_t stream);
 
-/* Gradient exchange of the multi-view step over NVLink peer memory (csrc/peer_exchange.cu; BASELINE config 4 / SURVEY.md 8e; the
- * reference has no multi-GPU step — this replaces the dist.all_gather + dist.all_reduce pair of the NCCL exchange).  One process
- * per GPU: adb_peer_alloc gives a zeroed device region, adb_peer_export its 64-byte CUDA IPC handle (exchanged by the host),
- * adb_peer_import maps another rank's region with peer access.  `*_ptrs` are HOST arrays of `world` (<= 8) device pointers, entry
- * r = the region (plus an offset) of rank r, the caller's own included.  All remote traffic is stores.
- *   adb_peer_signal        fence.sys, then flags_r[slot][rank] = value on every rank r (flags: unsigned [n_slots][8] per rank)
- *   adb_peer_wait          spins until local flags[slot][r] >= value for r < world and slot in [slot_lo, slot_lo+n_slots); after
- *                          timeout_s seconds it sets *err (device int) = 1 + slot instead of hanging the GPU
- *   adb_peer_push_rgb      colour gradient of one view masked by the SH clamp (splats[i].rgb > 0 ? v_splats[i][6:9] : 0) written
- *                          as row `row_off` (floats, multiple of 4) of every rank's table; campos[3] -> cam_ptrs[r] + cam_off
- *   adb_peer_bcast         a ready-made row of n_floats (multiple of 4) to every rank
- *   adb_peer_scatter       reduce-scatter by push: float4 i of src goes to slot `rank` of rank (i / per4)'s staging area
- *   adb_peer_reduce_bcast  the owner sums its shard's `world` slots in rank order and writes the sums to every rank's result */
-int adb_peer_warmup(void); /* loads the kernels below (lazy module loading must not happen while a wait kernel spins) */
-int adb_peer_alloc(size_t bytes, void** ptr /*HOST out*/);
-int adb_peer_free(void* ptr);
-int adb_peer_export(void* ptr, unsigned char* handle64 /*HOST out*/);
-int adb_peer_import(const unsigned char* handle64 /*HOST*/, void** ptr /*HOST out*/);
-int adb_peer_close(void* ptr);
-int adb_peer_signal(void* const* flag_ptrs /*HOST*/, int world, int slot, int rank, unsigned value, adb_stream_t stream);
-int adb_peer_wait(const void* local_flags, int world, int slot_lo, int n_slots, unsigned value, double timeout_s, int* err,
-                  adb_stream_t stream);
-int adb_peer_push_rgb(int N, const float* splats, const float* v_splats, void* const* dst_ptrs /*HOST*/, int world, size_t row_off,
-                      const float* campos, void* const* cam_ptrs /*HOST*/, size_t cam_off, adb_stream_t stream);
-int adb_peer_bcast(size_t n_floats, const float* src, void* const* dst_ptrs /*HOST*/, int world, size_t off_floats,
-                   const float* campos, void* const* cam_ptrs /*HOST*/, size_t cam_off, adb_stream_t stream);
-int adb_peer_scatter(size_t n4, size_t per4, const float* src, void* const* stage_ptrs /*HOST*/, int world, int rank,
-                     adb_stream_t stream);
-int adb_peer_reduce_bcast(size_t n4, size_t per4, const float* stage, void* const* out_ptrs /*HOST*/, int world, int rank,
-                          adb_stream_t stream);
-
 #ifdef __cplusplus
 }
 #endif
