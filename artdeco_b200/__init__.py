@@ -17,11 +17,12 @@ Public operators (same names / argument meaning as the reference's, see each mod
   keyframe.dense_point, keyframe.mapper_keyframe       (Backend.prepare_for_mapper + Keyframe.__init__: the key-frame hand-off)
   factor_graph.FactorGraph                             (VSLAM/mast3r_slam/global_opt.py: the Backend's factor graph)
   evaluate.evaluate, lpips.LPIPSVGG                    (SceneModel.evaluate: held-out PSNR, SSIM and LPIPS-VGG)
+  pi3.Pi3, pi3.accurate_loop_closure                  (Pi3 and RetrievalDatabase.accurate_loop_closure: the Backend's loop closure)
 There is no CPU implementation: every operator raises unless a CUDA sm_90 device and the C-ABI library
 ``libartdeco_b200.so`` are available.
 """
 from . import _lib  # noqa: F401
-from . import adam, covmlp, cull, densify, evaluate, factor_graph, gn, keyframe, knn, legacy, lpips, mapper, mast3r, matching, multiview, optimizers, parallel, raster, reanchor, scene, tracking, voxel  # noqa: F401  (each registers its C signatures)
+from . import adam, covmlp, cull, densify, evaluate, factor_graph, gn, keyframe, knn, legacy, lpips, mapper, mast3r, matching, multiview, optimizers, parallel, pi3, raster, reanchor, scene, tracking, voxel  # noqa: F401  (each registers its C signatures)
 from .adam import adamUpdate, adamUpdateBasic  # noqa: F401
 from .covmlp import cov_mlp_modulate  # noqa: F401
 from .cull import lod_cull, lod_select, weed_out_mask  # noqa: F401

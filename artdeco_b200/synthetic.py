@@ -82,6 +82,12 @@ def det_weights(shapes: dict, seed: int = 0, device="cpu"):
         return dict(ex.map(one, list(shapes.items())))
 
 
+def pi3_frames(N: int = 2, H: int = 392, W: int = 518, seed: int = 0):
+    """Pi3's input [1, N, 3, H, W] in [0, 1]."""
+    g = torch.Generator().manual_seed(seed)
+    return torch.rand(1, N, 3, H, W, generator=g)
+
+
 def mast3r_pair(B: int = 1, H: int = 512, W: int = 512, seed: int = 0):
     g = torch.Generator().manual_seed(seed)
     return (torch.rand(B, 3, H, W, generator=g) * 2 - 1, torch.rand(B, 3, H, W, generator=g) * 2 - 1)

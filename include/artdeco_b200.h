@@ -618,6 +618,40 @@ int adb_upsample2x_nhwc(int B, int Hin, int Win, int C, int Hout, int Wout, cons
 int adb_head_postprocess(int B, int H, int W, const float* pts, const float* lf, long long ld_lf, int n_desc, float* pts3d,
                          float* conf, float* desc, float* desc_conf, adb_stream_t stream);
 
+/* ---- Pi3 (the Backend's accurate loop closure) ----
+ * Paths under VSLAM/thirdparty/Pi3/pi3/models/ unless stated.  The dense layers run on adb_gemm_bf16 (act 2 = the camera
+ * head's ReLU) and adb_attention_bf16; these are the Pi3-specific stages.  H and W must be multiples of 14 and at
+ * least 14, every count of frames or views at least 1; misaligned pointers are refused before any launch.
+ * adb_pi3_patch14      (imgs - image_mean) / image_std (pi3.py:174) + the 14x14/s14 patch-embedding conv's operand
+ *                      (dinov2/layers/patch_embed.py:75): img [BN,3,H,W] in [0,1] -> bf16 split [BN*(H/14)*(W/14), 592],
+ *                      columns in (c, ky, kx) order, 588..591 zero.  hi/lo 16-byte aligned, lo may be NULL.
+ * adb_pi3_tokens       dinov2/models/vision_transformer.py:215-234: x [BN, 5+n, C] = [cls + pos[0], 4 registers,
+ *                      patch + pos[1..n]]; patch [BN*n, C], cls [C], reg [4, C], pos [1+n, C] (the interpolated table).
+ * adb_qknorm_rope      layers/attention.py:326-334: q or k of one qkv row block (columns col0 .. col0 + 64h of x fp32
+ *                      [B*N, ld]) -> optional per-head LayerNorm(64, eps) (gamma = beta = NULL skips it), RoPE2D base 100
+ *                      (layers/pos_embed.py:111-158; table as adb_rope_heads), bf16 split [B, h, N, 64].
+ * adb_pi3_point_head   pi3.py:193-209 + transformer_head.py:70-80: pts [BN*hw, 588] and cf [BN*hw, 196] (LinearPts3d GEMM
+ *                      outputs; the first `skip` rows of each view are register tokens), pose [BN,4,4] -> points,
+ *                      local_points [BN,H,W,3], conf [BN,H,W].
+ * adb_pi3_camera_tail  layers/camera_head.py:54-61: average pool of feat [BN*hw, 512] rows skip..hw-1, the more_mlps
+ *                      (w0t, w2t transposed [in][out]), fc_t and fc_rot in fp32 -> rot [BN, 9], trans [BN, 3].
+ * adb_pi3_svd_pose     layers/camera_head.py:66-93: R = V diag(1,1,det(V U^T)) U^T of the row-normalised rot^T, fp64 Jacobi;
+ *                      pose [BN,4,4] = [R t; 0 1] (trans NULL: t = 0).
+ * adb_pi3_window_input mast3r_slam/retrieval_database.py:21-41,268-270: img [N,3,Hi,Wi] in [-1,1] -> clamp(x/2 + 1/2, 0, 1)
+ *                      bilinearly resized (align_corners=False, no antialias) to out [N,3,Ho,Wo]. */
+int adb_pi3_patch14(int BN, int H, int W, const float* img, void* hi, void* lo, adb_stream_t stream);
+int adb_pi3_tokens(int BN, int n, int C, const float* patch, const float* cls, const float* reg, const float* pos, float* x,
+                   adb_stream_t stream);
+int adb_qknorm_rope(int B, int N, int h, long long ld, int col0, const float* x, const float* gamma, const float* beta,
+                    float eps, const long long* pos, const float* table, int n_pos, void* hi, void* lo, adb_stream_t stream);
+int adb_pi3_point_head(int BN, int H, int W, int hw, int skip, const float* pts, const float* cf, const float* pose,
+                       float* points, float* local_points, float* conf, adb_stream_t stream);
+int adb_pi3_camera_tail(int BN, int hw, int skip, const float* feat, const float* w0t, const float* b0, const float* w2t,
+                        const float* b2, const float* wt, const float* bt, const float* wr, const float* br, float* rot,
+                        float* trans, adb_stream_t stream);
+int adb_pi3_svd_pose(int BN, const float* rot, const float* trans, float* pose, adb_stream_t stream);
+int adb_pi3_window_input(int N, int Hi, int Wi, const float* img, int Ho, int Wo, float* out, adb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
