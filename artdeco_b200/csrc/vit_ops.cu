@@ -194,7 +194,7 @@ softmax_reg_kernel(long long rows, int L, long long ld_in, long long ld_out, con
     if (row >= rows) return;
     const float* sr = s + (size_t)row * ld_in;
     float v[CH][4];
-    float m = -3.0e38f;
+    float m = -INFINITY;          // not a finite floor: a row of finfo.min logits would underflow every term to 0
 #pragma unroll
     for (int k = 0; k < CH; ++k) {
         const int c = k * 128 + lane * 4;
@@ -244,7 +244,7 @@ softmax_kernel(long long rows, int L, long long ld_in, long long ld_out, const f
     const int lane = threadIdx.x & 31;
     if (row >= rows) return;
     const float* sr = s + (size_t)row * ld_in;
-    float m = -3.0e38f;
+    float m = -INFINITY;
     for (int c = lane; c < L; c += 32) m = fmaxf(m, sr[c]);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
@@ -272,6 +272,9 @@ im2col_patch_kernel(int B, int H, int W, const float* __restrict__ img, __nv_bfl
 }
 
 inline int grid_for(long long n) { long long g = (n + 255) / 256; return (int)(g < 132LL * 32 ? g : 132LL * 32); }
+
+// NULL passes: optional outputs are checked only when given
+inline bool aligned(const void* p, unsigned bytes) { return ((uintptr_t)p % bytes) == 0; }
 
 }  // namespace
 
@@ -368,6 +371,8 @@ ADB_API int adb_layernorm(long long rows, int C, const float* x, const float* ga
     ADB_REQUIRE(rows >= 0 && C >= 8 && C <= 2048 && C % 8 == 0, "adb_layernorm: C must be a multiple of 8 in [8, 2048]");
     if (rows == 0) return ADB_OK;
     ADB_REQUIRE(x && gamma && beta && (y || y_hi), "adb_layernorm: null pointer");
+    ADB_REQUIRE(aligned(x, 16) && aligned(gamma, 16) && aligned(beta, 16) && aligned(y, 16) && aligned(y_hi, 16) &&
+                    aligned(y_lo, 16), "adb_layernorm: x, gamma, beta, y, y_hi and y_lo must be 16-byte aligned");
     const int blocks = (int)((rows + 7) / 8);
     if (C <= 1024)
         layernorm_kernel<4><<<blocks, 256, 0, stream>>>(rows, C, x, gamma, beta, eps, y, (__nv_bfloat16*)y_hi, (__nv_bfloat16*)y_lo);
@@ -391,7 +396,10 @@ ADB_API int adb_rope_heads(int B, int N, int h, long long ld, int col0, const fl
     ADB_REQUIRE(B >= 0 && N >= 0 && h >= 1 && mode >= 0 && mode <= 2, "adb_rope_heads: bad args");
     if ((long long)B * N == 0) return ADB_OK;
     ADB_REQUIRE(x && hi && (mode != 0 || (pos && table && n_pos > 0)), "adb_rope_heads: null pointer");
+    ADB_REQUIRE(col0 >= 0 && ld >= (long long)col0 + h * 64, "adb_rope_heads: need ld >= col0 + h*64");
     ADB_REQUIRE(ld % 4 == 0 && col0 % 4 == 0 && ((uintptr_t)x % 16 == 0), "adb_rope_heads: x must allow 128-bit loads");
+    ADB_REQUIRE(aligned(hi, 16) && aligned(lo, 16) && aligned(pos, 8) && aligned(table, 8),
+                "adb_rope_heads: hi and lo must be 16-byte aligned, pos and table 8-byte aligned");
     if (mode == 2) {
         ADB_REQUIRE(Npad >= N && Npad % 8 == 0, "adb_rope_heads: Npad must be a multiple of 8 and >= N");
         dim3 grid(adb_cdiv(Npad, 64), h, B);
@@ -486,6 +494,8 @@ ADB_API int adb_upsample2x_nhwc(int B, int Hin, int Win, int C, int Hout, int Wo
     if (B == 0) return ADB_OK;
     ADB_REQUIRE(x && (y || hi), "adb_upsample2x_nhwc: null pointer");
     ADB_REQUIRE(!lo || hi, "adb_upsample2x_nhwc: lo without hi");
+    ADB_REQUIRE(aligned(x, 16) && aligned(addend, 16) && aligned(y, 16) && aligned(hi, 8) && aligned(lo, 8),
+                "adb_upsample2x_nhwc: x, addend and y must be 16-byte aligned, hi and lo 8-byte aligned");
     upsample2x_kernel<<<grid_for((long long)B * Hout * Wout * (C / 4)), 256, 0, stream>>>(
         B, Hin, Win, C, Hout, Wout, x, addend, y, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo);
     ADB_CHECK_LAUNCH("upsample2x_kernel");
@@ -501,6 +511,8 @@ ADB_API int adb_head_postprocess(int B, int H, int W, const float* pts, const fl
     ADB_REQUIRE(n_desc == 24, "adb_head_postprocess: only the desc24 head (output_mode pts3d+desc24) is built");
     if (B == 0) return ADB_OK;
     ADB_REQUIRE(pts && lf && pts3d && conf && desc && desc_conf, "adb_head_postprocess: null pointer");
+    ADB_REQUIRE(aligned(pts, 16) && aligned(desc, 16) && aligned(lf, 4) && aligned(pts3d, 4) && aligned(conf, 4) &&
+                    aligned(desc_conf, 4), "adb_head_postprocess: pts and desc must be 16-byte aligned, the rest 4-byte aligned");
     head_postprocess_kernel<24><<<grid_for((long long)B * H * W), 256, 0, stream>>>(B, H, W, pts, lf, ld_lf, pts3d, conf,
                                                                                    desc, desc_conf);
     ADB_CHECK_LAUNCH("head_postprocess_kernel");

@@ -555,10 +555,14 @@ int adb_knn_index(long long P, const float* points, int K, long long Q, const in
  *    mast3r/catmlp_dpt_head.py:67-69): D[z] = act(alpha * A[z] * B[z]^T + bias) + residual[z],
  *   A bf16 [batch][M][K], B bf16 [batch][N][K], both K-contiguous; *_lo != NULL selects the 3-term bf16x3 product;
  *   outputs fp32 D and/or a bf16 (hi, lo) split; output offset = (z / zdiv) * s?2 + (z % zdiv) * s? (zdiv <= 0: z * s?).
- * adb_layernorm     nn.LayerNorm(eps) rows of C (croco.py:34, blocks.py:127-130,186-191)
+ * adb_layernorm     nn.LayerNorm(eps) rows of C (croco.py:34, blocks.py:127-130,186-191); C a multiple of 8 in [8, 2048];
+ *                   x, gamma, beta, y, y_hi, y_lo 16-byte aligned (y or y_hi may be NULL, y_lo NULL gives hi only)
  * adb_rope_heads    RoPE2D + head split (pos_embed.py:112-159 / curope/kernels.cu:18-82): x fp32 [B,N,ld] -> bf16 split
- *                   [B,h,N,64] (mode 0 RoPE, 1 plain) or transposed [B,h,64,Npad] (mode 2)
- * adb_softmax_rows  attn.softmax(-1) (blocks.py:106,163), fp32 in, bf16 split out
+ *                   [B,h,N,64] (mode 0 RoPE, 1 plain) or transposed [B,h,64,Npad] (mode 2, Npad a multiple of 8, pad
+ *                   columns written as 0).  ld >= col0 + h*64, ld and col0 multiples of 4; x, hi, lo 16-byte aligned,
+ *                   pos and table 8-byte aligned.  Positions outside [0, n_pos) are clamped to the nearest table row.
+ * adb_softmax_rows  attn.softmax(-1) (blocks.py:106,163), fp32 in, bf16 split out; columns L..ld_out-1 are not written.
+ *                   Any alignment (a misaligned or strided row takes the generic kernel); all -inf or NaN rows give NaN
  * adb_im2col_patch16  operand of the 16x16/s16 patch-embedding conv as a GEMM (patch_embed.py:19-29)
  * adb_split_bf16    x -> (hi = rn(x), lo = rn(x - hi)) */
 int adb_gemm_bf16(int batch, int M, int N, int K, const void* A_hi, const void* A_lo, long long lda, long long sA,
@@ -612,7 +616,8 @@ int adb_im2col_patch16(int B, int H, int W, const float* img, void* hi, void* lo
  * the crop of dpt_head.py:57 (Hout <= 2 Hin) and the bf16 split the next conv consumes; y / (hi, lo) may each be NULL.
  * adb_head_postprocess: pixel_shuffle(16) + concat + postprocess of mast3r/catmlp_dpt_head.py:25-39,87-96 and
  * dust3r/heads/postprocess.py:22-58 in one pass: pts [B,H,W,4] (DPT map) + lf [B*(H/16)*(W/16), ld_lf] (local-feature MLP
- * output before the pixel shuffle, 25*256 columns) -> pts3d [B,H,W,3], conf [B,H,W], desc [B,H,W,24], desc_conf [B,H,W]. */
+ * output before the pixel shuffle, 25*256 columns) -> pts3d [B,H,W,3], conf [B,H,W], desc [B,H,W,24], desc_conf [B,H,W].
+ * Alignment: upsample x, addend, y 16 bytes and hi, lo 8 bytes; head_postprocess pts and desc 16 bytes, the rest 4. */
 int adb_upsample2x_nhwc(int B, int Hin, int Win, int C, int Hout, int Wout, const float* x, const float* addend, float* y,
                         void* hi, void* lo, adb_stream_t stream);
 int adb_head_postprocess(int B, int H, int W, const float* pts, const float* lf, long long ld_lf, int n_desc, float* pts3d,

@@ -96,6 +96,18 @@ def test_cuda_model_matches_reference_golden_full(cuda):
 
 
 @pytest.mark.gpu
+def test_every_weight_the_model_passes_is_16_byte_aligned(cuda):
+    """adb_layernorm reads gamma and beta with 128-bit loads and refuses misaligned pointers, so every fp32 parameter and
+    every bf16 weight split the model holds must start on a 16-byte boundary."""
+    from artdeco_b200.mast3r import AsymmetricMASt3R
+    cfg = mt.SMALL_CFG
+    m = AsymmetricMASt3R(**cfg).load_state_dict(synthetic.det_weights(mt.param_shapes(cfg))).to(cuda)
+    bad = [k for k, v in m._sd.items() if v.data_ptr() % 16]
+    bad += [k for k, s in m._w.items() for t in (s.hi, s.lo) if t is not None and t.data_ptr() % 16]
+    assert len(m._sd) > 100 and not bad, bad
+
+
+@pytest.mark.gpu
 def test_graphed_bench_batch_replay_matches_golden_and_eager(cuda):
     """The configuration bench.py times: GraphedForwardPair(model, BENCH_PAIRS_PER_GPU, 512, 512) on two streams, REPLAYED (the race fixed
     in round 1 only showed under replay).  Batch item 0 is the golden pair, so all four outputs of both views are checked

@@ -143,6 +143,14 @@ def test_qknorm_rope_against_float64():
         assert rel(got, want) < 1e-5, rel(got, want)
 
 
+def test_every_weight_the_model_passes_is_16_byte_aligned(model):
+    """adb_layernorm and adb_pi3_tokens read their parameters with 128-bit loads and refuse misaligned pointers, so every
+    fp32 parameter and every bf16 weight split the model holds must start on a 16-byte boundary."""
+    bad = [k for k, v in model._sd.items() if v.data_ptr() % 16]
+    bad += [k for k, s in model._w.items() for t in (s.hi, s.lo) if t is not None and t.data_ptr() % 16]
+    assert len(model._sd) > 100 and not bad, bad
+
+
 # ---- accurate loop closure --------------------------------------------------------------------------------------
 CFG = {"matching": dict(max_iter=10, lambda_init=1e-8, convergence_thresh=1e-6, dist_thresh=1e-1, radius=4, dilation_max=5),
        "retrieval": dict(accurate_min=0.15, k=3)}
