@@ -28,6 +28,8 @@
 #include "hopper.cuh"
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <limits.h>
+#include <math.h>
 #include <stdio.h>
 
 namespace {
@@ -68,6 +70,10 @@ struct GemmParams {
     const long long* rope_pos;      // int64 [M, 2] (y, x)
     const float* rope_table;        // [n_pos][16][2] (cos, sin)
     __nv_bfloat16* rope_hi[2]; __nv_bfloat16* rope_lo[2];
+    // top-MA epilogue (adb_retrieval_assign): dist = (qn[row] + cn[col]) - 2 acc; per row and N-tile, the MA smallest
+    // (dist, col), smaller col first among equal distances, go to cand_d / cand_i [M][tiles_n][ma]
+    const float* qn; const float* cn; int ma;
+    float* cand_d; int* cand_i;
 };
 
 __device__ __forceinline__ float gelu_erf(float v) { return 0.5f * v * (1.0f + erff(v * 0.70710678118654752f)); }
@@ -221,7 +227,62 @@ __device__ __forceinline__ void store_row(const GemmParams& p, float (&acc)[2][3
     }
 }
 
-template <bool ROPE>
+// (distance, column) strictly before in the order "smaller distance first, then smaller column"
+__device__ __forceinline__ bool topma_before(float da, int ia, float db, int ib) { return da < db || (da == db && ia < ib); }
+
+// Epilogue of adb_retrieval_assign: the thread's 64 columns of output row `trow` -> its sorted top 8 in (bd, bi); the
+// two threads of a row (half 0 and 1) then merge through `xch`, and half 0 writes the row's MA candidates of this N-tile.
+__device__ __forceinline__ void topma_row(const GemmParams& p, float (&acc)[2][32], int trow, int half, int m0, int n0,
+                                          int nt, int tiles_n, float* xch) {
+    const int row = m0 + trow;
+    float bd[8];
+    int bi[8];
+#pragma unroll
+    for (int q = 0; q < 8; ++q) { bd[q] = INFINITY; bi[q] = INT_MAX; }
+    if (row < p.M) {
+        const float qn = __ldg(p.qn + row);
+#pragma unroll
+        for (int g = 0; g < 2; ++g)
+#pragma unroll
+            for (int j = 0; j < 32; ++j) {
+                const int col = n0 + half * 64 + g * 32 + j;
+                if (col >= p.N) continue;
+                // torch: (sum(q**2)[:, None] + sum(c**2)[None, :]) - 2 * (q @ c.T), all fp32
+                const float d = __fsub_rn(__fadd_rn(qn, __ldg(p.cn + col)), __fmul_rn(2.f, acc[g][j]));
+                if (!(d < bd[7])) continue;          // columns ascend: an equal distance never displaces an earlier one
+#pragma unroll
+                for (int q = 7; q >= 1; --q) {
+                    if (d < bd[q - 1]) { bd[q] = bd[q - 1]; bi[q] = bi[q - 1]; }
+                    else if (d < bd[q]) { bd[q] = d; bi[q] = col; }
+                }
+                if (d < bd[0]) { bd[0] = d; bi[0] = col; }
+            }
+    }
+    float* xd = xch + trow * 16;
+    int* xi = reinterpret_cast<int*>(xd + 8);
+    if (half == 1) {
+#pragma unroll
+        for (int q = 0; q < 8; ++q) { xd[q] = bd[q]; xi[q] = bi[q]; }
+    }
+    asm volatile("bar.sync 1, %0;" ::"n"(NCONSUMER) : "memory");
+    if (half == 1 || row >= p.M) return;
+    float* od = p.cand_d + ((size_t)row * tiles_n + nt) * p.ma;
+    int* oi = p.cand_i + ((size_t)row * tiles_n + nt) * p.ma;
+    int a = 0, b = 0;
+    for (int r = 0; r < p.ma; ++r) {
+        float da = INFINITY, db = INFINITY;
+        int ia = INT_MAX, ib = INT_MAX;
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+            if (q == a) { da = bd[q]; ia = bi[q]; }
+            if (q == b) { db = xd[q]; ib = xi[q]; }
+        }
+        if (topma_before(db, ib, da, ia)) { od[r] = db; oi[r] = ib; ++b; }
+        else { od[r] = da; oi[r] = ia; ++a; }
+    }
+}
+
+template <bool ROPE, bool TOPMA = false>
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_constant__ CUtensorMap mapAlo,
                const __grid_constant__ CUtensorMap mapBhi, const __grid_constant__ CUtensorMap mapBlo,
@@ -351,6 +412,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_constant
             const float4 v = *reinterpret_cast<const float4*>(stg + trow * STG_LD + half * 64 + g * 32 + j);
             out[g][j] = v.x; out[g][j + 1] = v.y; out[g][j + 2] = v.z; out[g][j + 3] = v.w;
         }
+    if constexpr (TOPMA) {
+        asm volatile("bar.sync 1, %0;" ::"n"(NCONSUMER) : "memory");   // every row is read out of the staging tile
+        topma_row(p, out, trow, half, m0, n0, tc.nt, tiles_n, stg);
+        return;
+    }
     const int zo = tc.bz / p.zdiv, zi = tc.bz % p.zdiv;
     const size_t dbase = (size_t)zo * p.sD2 + (size_t)zi * p.sD;
     const size_t obase = (size_t)zo * p.sO2 + (size_t)zi * p.sO;
@@ -407,11 +473,13 @@ int launch(const CUtensorMap& mAhi, const CUtensorMap& mAlo, const CUtensorMap& 
         const int rc = once.ensure([]() -> int {
             ADB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
             ADB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+            ADB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
             return ADB_OK;
         });
         if (rc != ADB_OK) return rc;
     }
-    if (p.rope_ndst > 0) gemm_tc_kernel<true><<<(unsigned)num_tiles, NTHREADS, SMEM_BYTES, stream>>>(mAhi, mAlo, mBhi, mBlo, p);
+    if (p.cand_d) gemm_tc_kernel<false, true><<<(unsigned)num_tiles, NTHREADS, SMEM_BYTES, stream>>>(mAhi, mAlo, mBhi, mBlo, p);
+    else if (p.rope_ndst > 0) gemm_tc_kernel<true><<<(unsigned)num_tiles, NTHREADS, SMEM_BYTES, stream>>>(mAhi, mAlo, mBhi, mBlo, p);
     else gemm_tc_kernel<false><<<(unsigned)num_tiles, NTHREADS, SMEM_BYTES, stream>>>(mAhi, mAlo, mBhi, mBlo, p);
     ADB_CHECK_LAUNCH("gemm_tc_kernel");
     return ADB_OK;
@@ -547,5 +615,32 @@ ADB_API int adb_conv3x3_bf16(int B, int H, int W, int Cin, int Cout, const void*
     p.conv_wb = wb; p.conv_hb = hb; p.conv_H = H; p.conv_W = W; p.conv_chunks = chunks;
     p.conv_tiles_x = adb_cdiv(W, wb); p.conv_tiles_y = adb_cdiv(H, hb);
     const long long tiles = (long long)p.conv_tiles_x * p.conv_tiles_y * adb_cdiv(Cout, BN) * B;
+    return launch(mAhi, mAlo, mBhi, mBlo, p, tiles, stream);
+}
+
+// Codebook assignment of adb_retrieval_assign's first launch (retrieval_database.py:355-367 quantize_custom): squared L2
+// distances of q [nq, D] to the centroids c [K, D] as (qn + cn) - 2 q c^T on the bf16x3 wgmma GEMM, reduced in the
+// epilogue of every 128-column tile to that tile's MA smallest (dist, index) per row: cand_d / cand_i [nq][cdiv(K,128)][MA].
+// The [nq, K] distance matrix is never written.  adb_retrieval_topma_merge reduces the tiles.
+ADB_API int adb_retrieval_assign(int nq, int K, int D, int MA, const void* q_hi, const void* q_lo, const void* c_hi,
+                                 const void* c_lo, const float* qn, const float* cn, float* cand_d, int* cand_i,
+                                 cudaStream_t stream) {
+    ADB_REQUIRE(nq >= 1 && K >= 1 && D >= 1 && MA >= 1 && MA <= 8 && MA <= K, "adb_retrieval_assign: need 1 <= MA <= min(8, K)");
+    ADB_REQUIRE(q_hi && q_lo && c_hi && c_lo && qn && cn && cand_d && cand_i, "adb_retrieval_assign: null pointer");
+    ADB_REQUIRE(D % 8 == 0, "adb_retrieval_assign: D must be a multiple of 8");
+    ADB_REQUIRE((((uintptr_t)q_hi | (uintptr_t)q_lo | (uintptr_t)c_hi | (uintptr_t)c_lo) % 16) == 0,
+                "adb_retrieval_assign: operands must be 16-byte aligned");
+    GemmParams p{};
+    p.nterms = 3;
+    CUtensorMap mAhi, mAlo, mBhi, mBlo;
+    int rc;
+    if ((rc = make_map(&mAhi, q_hi, nq, D, D, 0, 1))) return rc;
+    if ((rc = make_map(&mAlo, q_lo, nq, D, D, 0, 1))) return rc;
+    if ((rc = make_map(&mBhi, c_hi, K, D, D, 0, 1))) return rc;
+    if ((rc = make_map(&mBlo, c_lo, K, D, D, 0, 1))) return rc;
+    p.M = nq; p.N = K; p.K = D; p.batch = 1;
+    p.alpha = 1.0f; p.zdiv = 1 << 30;
+    p.qn = qn; p.cn = cn; p.ma = MA; p.cand_d = cand_d; p.cand_i = cand_i;
+    const long long tiles = (long long)adb_cdiv(nq, BM) * adb_cdiv(K, BN);
     return launch(mAhi, mAlo, mBhi, mBlo, p, tiles, stream);
 }

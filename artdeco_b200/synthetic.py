@@ -91,3 +91,95 @@ def pi3_frames(N: int = 2, H: int = 392, W: int = 518, seed: int = 0):
 def mast3r_pair(B: int = 1, H: int = 512, W: int = 512, seed: int = 0):
     g = torch.Generator().manual_seed(seed)
     return (torch.rand(B, 3, H, W, generator=g) * 2 - 1, torch.rand(B, 3, H, W, generator=g) * 2 - 1)
+
+
+# ---- key-frame retrieval (retrieval.RetrievalDatabase) ----
+# Descriptors are built in the whitened space: token t of a place is s_t * normalize(c_w + 0.5 g) for a random visual word
+# w, with attention norms s_t = 1 + 1e-3 * rank, so the attention order has 1e-3 relative gaps.  A revisit adds 0.05 of
+# fresh noise to every direction of the place.  Margins are measured in float64 on the fp32 encoder tokens; tokens whose
+# decision is too close to call in fp32 (attention order, the order of the assignment's MA + 1 nearest distances, the sign
+# of an aggregated residual component) are re-drawn until every margin clears its bound.
+RETRIEVAL_MARGIN_DIST = 2.0 ** -12      # consecutive gap of the MA + 1 nearest distances / (|d|^2 + |c|^2)
+RETRIEVAL_MARGIN_RESID = 2.0 ** -18     # |r_j| / sum |d_j - c_j| over the word's members
+RETRIEVAL_MARGIN_ATTN = 1e-5            # relative gap of consecutive attention norms, ranks 0..nfeat
+
+
+def retrieval_model(K: int, dim: int = 1024, seed: int = 0):
+    """(m [1, dim] float64, P [dim, dim] float64 orthogonal, centroids [K, dim] fp32 of unit norm)."""
+    g = torch.Generator().manual_seed(seed)
+    m = 0.01 * torch.randn(1, dim, generator=g, dtype=torch.float64)
+    P, _ = torch.linalg.qr(torch.randn(dim, dim, generator=g, dtype=torch.float64))
+    c = torch.randn(K, dim, generator=g, dtype=torch.float64)
+    return m, P, (c / c.norm(dim=1, keepdim=True)).float()
+
+
+def _retrieval_margins(x, m, P, cent, cn, nfeat, ma):
+    """float64 margins of one frame's fp32 tokens x [n, dim] -> (offending token ids, (attn, dist, resid) minima)."""
+    y = ((x.double() - m) @ P).float().double()
+    a = y.norm(dim=1)
+    order = torch.argsort(a, descending=True)
+    sel = order[:nfeat]
+    top = a[order[:nfeat + 1]]
+    ag = (top[:-1] - top[1:]) / top[:-1]
+    bad = set(order[:nfeat + 1][:-1][ag < RETRIEVAL_MARGIN_ATTN].tolist())
+    d = y[sel]
+    dist = (d * d).sum(1, keepdim=True) + cn[None, :] - 2.0 * d @ cent.T
+    sd, si = torch.sort(dist, dim=1)
+    scale = (d * d).sum(1) + cn[si[:, 0]]
+    dmin = ((sd[:, 1:ma + 1] - sd[:, :ma]) / scale[:, None]).min(1).values   # the order of the MA words and the MA+1-th
+    bad |= set(sel[dmin < RETRIEVAL_MARGIN_DIST].tolist())
+    rmin = float("inf")
+    for cols in (si[:, :1], si[:, :ma]):
+        words = torch.unique(cols)
+        for w in words.tolist():
+            rows = (cols == w).any(1)
+            diff = d[rows] - cent[w]
+            ratio = (diff.sum(0).abs() / diff.abs().sum(0).clamp_min(1e-300)).min()
+            rmin = min(rmin, float(ratio))
+            if ratio < RETRIEVAL_MARGIN_RESID:
+                bad |= set(sel[rows].tolist())
+    return bad, (float(ag.min()), float(dmin.min()), rmin)
+
+
+def retrieval_stream(m, P, centroids, schedule, n: int = 768, nfeat: int = 300, ma: int = 5, seed: int = 0):
+    """Key-frame encoder features for a schedule of (place, add_after_query) pairs: a place seen before is a revisit.
+    Returns a list of dicts {feat [1, n, dim] fp32, place, add, revisit, margins (attn, dist, resid)}."""
+    g = torch.Generator().manual_seed(seed + 1)
+    dim = P.shape[0]
+    cent = centroids.double()
+    cn = (cent * cent).sum(1)
+    places = {}
+    out = []
+    for place, add in schedule:
+        revisit = place in places
+        if not revisit:
+            perm = torch.randperm(n, generator=g)
+            words = torch.randint(0, cent.shape[0], (n,), generator=g)
+            places[place] = (1.0 + 1e-3 * perm.double(), words, torch.randn(n, dim, generator=g, dtype=torch.float64))
+        s, words, base = places[place]
+
+        def direction(rows):
+            noise = torch.randn(len(rows), dim, generator=g, dtype=torch.float64) / dim ** 0.5
+            v = cent[words[rows]] + 0.5 * base[rows] / dim ** 0.5
+            v = v / v.norm(dim=1, keepdim=True) + 0.05 * noise if revisit else v + 0.02 * noise
+            return v / v.norm(dim=1, keepdim=True) * s[rows, None]
+
+        yd = direction(torch.arange(n))
+        for _ in range(100):
+            x = ((yd @ P.T) + m).float()
+            bad, margins = _retrieval_margins(x, m, P, cent, cn, nfeat, ma)
+            if not bad:
+                break
+            rows = torch.tensor(sorted(bad))
+            yd[rows] = direction(rows)
+        else:
+            raise RuntimeError("retrieval_stream: margins did not clear in 100 re-draws")
+        out.append(dict(feat=x[None].contiguous(), place=place, add=add, revisit=revisit, margins=margins))
+    return out
+
+
+# 30 updates: 14 new places (the Pi3 gate is reached at 12), a short-range revisit (retrieval kept), long-range revisits
+# (Pi3), a relocalisation query later re-added, never-seen places (empty match) and a second lap.
+RETRIEVAL_SCHEDULE = ([(p, True) for p in range(14)] + [(13, True), (1, True), (5, False), (5, True), (100, True),
+                      (2, True), (14, True), (15, True), (14, True), (101, False), (3, True), (16, True), (0, True),
+                      (17, True), (6, True), (9, True)])

@@ -657,6 +657,49 @@ int adb_pi3_camera_tail(int BN, int hw, int skip, const float* feat, const float
 int adb_pi3_svd_pose(int BN, const float* rot, const float* trans, float* pose, adb_stream_t stream);
 int adb_pi3_window_input(int N, int Hi, int Wi, const float* img, int Ho, int Wo, float* out, adb_stream_t stream);
 
+/* ---- Key-frame retrieval (the Backend's loop-candidate query) ----
+ * VSLAM/mast3r_slam/retrieval_database.py with the trainingfree retrieval model (prewhiten only, l2norm attention, binary
+ * ASMK, MA <= 8); paths under VSLAM/thirdparty/mast3r/ unless stated.  No call synchronises.
+ * adb_retrieval_whiten        mast3r/retrieval/model.py:55-76 Whitener + :88-109 attention: y [n,D] = fp32((double(x) - m) P)
+ *                             with an fp64 FMA GEMM, attn [n] = fp32 ||y||_2 of the fp32 row.
+ * adb_retrieval_select        model.py:113-135 how_select_local's topk: tok [nfeat] = token ids by attention, descending,
+ *                             ties to the lower id (n <= 1024).
+ * adb_retrieval_gather_split  dst [rows,D] = src[tok[r]] (tok NULL: identity, dst may be NULL), its bf16 (hi, lo) split and
+ *                             fp32 squared norm sqn [rows]: the query descriptors, and the centroids once at load.
+ * adb_retrieval_assign        retrieval_database.py:355-367 quantize_custom on the bf16x3 wgmma GEMM (csrc/gemm_tc.cu):
+ *                             per row and 128-column tile, the MA smallest (qn + cn) - 2 q.c with their indices ->
+ *                             cand_d, cand_i [nq][cdiv(K,128)][MA]; hi/lo 16-byte aligned, D % 8 == 0, MA <= min(8, K).
+ * adb_retrieval_topma_merge   the tiles' candidates -> words [nq, MA], ascending distance, ties to the lower index.
+ * adb_retrieval_aggregate     asmk/kernel.py:26-39 aggregate_image + asmk/cython/hamming.pyx:90-117 binarize_and_pack_2D:
+ *                             the words[r*ld + c] (c < MA) -> out_words (sorted unique, *out_count of them) and out_sig
+ *                             [count, D/32] (bit 31-j of word w = sum_r (desc[r] - centroid)[32w+j] > 0, fp32, descriptor
+ *                             order).  nfeat*MA <= 8192, D a multiple of 32 up to 1024.  Written into row i of the device
+ *                             inverted file, it is the append (asmk/inverted_file.py:56-83).
+ * adb_retrieval_search        asmk/inverted_file.py:86-112 + kernel.py:56-70 + functional.py:11-15: scores [n_db] (float64)
+ *                             of the query (q_words sorted, q_sig, *q_count) against the image-major inverted file
+ *                             (db_words [n_db, nfeat] sorted, db_sig [n_db, nfeat, nw], db_count [n_db]); pow_table
+ *                             [16 nw + 1] = float32 (1 - 2 p/(32 nw))**alpha for popcount p, built on the host.
+ * adb_retrieval_rank          retrieval_database.py:224-247,263-267: out[0] = n_valid, out[1..k] = the top-k ids whose
+ *                             score > min_thresh (ties to the lower id), out[k+1] = the lowest of them (-1: none),
+ *                             out[k+2] = min(window, n_db), out[k+3..] = ids by descending float64 score*100, ties to the
+ *                             lower id (the stable sort of the similarity-graph row). */
+int adb_retrieval_whiten(int n, int D, const float* x, const double* m, const double* P, float* y, float* attn,
+                         adb_stream_t stream);
+int adb_retrieval_select(int n, int nfeat, const float* attn, int* tok, adb_stream_t stream);
+int adb_retrieval_gather_split(long long rows, int D, const float* src, const int* tok, float* dst, void* hi, void* lo,
+                               float* sqn, adb_stream_t stream);
+int adb_retrieval_assign(int nq, int K, int D, int MA, const void* q_hi, const void* q_lo, const void* c_hi, const void* c_lo,
+                         const float* qn, const float* cn, float* cand_d, int* cand_i, adb_stream_t stream);
+int adb_retrieval_topma_merge(int nq, int ntiles, int MA, const float* cand_d, const int* cand_i, int* words,
+                              adb_stream_t stream);
+int adb_retrieval_aggregate(int nfeat, int D, int MA, int ld, const float* desc, const int* words, const float* centroids,
+                            int* out_words, unsigned* out_sig, int* out_count, adb_stream_t stream);
+int adb_retrieval_search(int n_db, int nfeat, int nw, const int* q_words, const unsigned* q_sig, const int* q_count,
+                         const int* db_words, const unsigned* db_sig, const int* db_count, const float* pow_table,
+                         double* scores, adb_stream_t stream);
+int adb_retrieval_rank(int n_db, const double* scores, int k, double min_thresh, int window, long long* out,
+                       adb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
